@@ -116,6 +116,20 @@ public:
   }
 #endif
 
+  // Keyframe depth prior (rmd_seeds_set_prior_propagation / rmd_seeds_propagate_prior, include/rmd_b200.h):
+  // in place, every later setReferenceImage starts from this keyframe's converged seeds (0 = off) ...
+  void setPriorPropagation(float sigma_sq_frac)
+  {
+    detail::throw_on_error(rmd_seeds_set_prior_propagation(handle_, sigma_sq_frac),
+                           "SeedMatrix: unable to set the prior propagation");
+  }
+  // ... or, right after setReferenceImage, from the converged seeds of another live keyframe.
+  void propagatePriorFrom(const SeedMatrix &src, float sigma_sq_frac)
+  {
+    detail::throw_on_error(rmd_seeds_propagate_prior(handle_, src.handle_, sigma_sq_frac),
+                           "SeedMatrix: unable to propagate the prior");
+  }
+
   // The C-ABI handle, for rmd::DepthmapDenoiser and code that wants the
   // extended entry points (u8 frames, device-resident frames, streams).
   rmd_seeds_t *handle() const { return handle_; }

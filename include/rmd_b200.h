@@ -167,6 +167,33 @@ int rmd_seeds_set_reference_u8(rmd_seeds_t *s, const uint8_t *host_img,
                                const float *T_curr_world, float min_depth,
                                float max_depth);
 
+/* Depth prior of a new keyframe from the converged seeds of another one (the
+ * reference starts every keyframe from the uniform prior; DESIGN.md 4.7).
+ * Every CONVERGED seed of the source is back-projected exactly as
+ * rmd_seeds_point_cloud does, moved into the new reference view, and splatted
+ * to the nearest pixel (the nearest surface wins; points behind the camera,
+ * outside [min_depth, max_depth] or outside the image are dropped).  After the
+ * usual initialisation, every non-BORDER pixel that received a point gets the
+ * seed (distance, sigma_sq_frac * range^2 / 36, 10, 10); all others keep the
+ * uniform prior.  The state stays UPDATE: new frames still have to confirm it.
+ *
+ * In place, for the reference's single-Depthmap node: with f > 0, every later
+ * set_reference* on s (float, u8 with or without undistortion, device) first
+ * splats s's own CONVERGED seeds of the keyframe it is leaving into the new
+ * reference view, then initialises, then applies the prior.  f = 0 (the
+ * default) switches it off.  f must be in [0, 1]. */
+int rmd_seeds_set_prior_propagation(rmd_seeds_t *s, float sigma_sq_frac);
+
+/* Cross-handle, for a set of live keyframes: dst has just had set_reference*
+ * and no update since; its seeds receive the prior splatted from src's current
+ * state (f in (0, 1]).  Image sizes and cameras may differ; the device must be
+ * the same.  Asynchronous, ordered on the device like
+ * rmd_denoiser_run_seeds_to_device: a later update of src does not overwrite
+ * seeds the splat is still reading.  Returns RMD_ERR_NOT_INITIALISED if dst
+ * has no reference or has been updated since it was set, or if src has no
+ * reference.  A source without CONVERGED seeds leaves dst's initial state. */
+int rmd_seeds_propagate_prior(rmd_seeds_t *dst, const rmd_seeds_t *src, float sigma_sq_frac);
+
 /* SeedMatrix::update, seed_matrix.cu:120-158: convergence check, epipolar NCC
  * search, triangulation and Bayesian update of every seed -- one fused kernel.
  * The host buffer may be reused as soon as the call returns (it is copied to

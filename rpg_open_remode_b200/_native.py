@@ -30,6 +30,8 @@ _SIGNATURES = {
     "rmd_seeds_set_reference": (ci, [vp, vp, vp, cf, cf]),
     "rmd_seeds_set_reference_device": (ci, [vp, vp, cs, vp, cf, cf]),
     "rmd_seeds_set_reference_u8": (ci, [vp, vp, vp, cf, cf]),
+    "rmd_seeds_set_prior_propagation": (ci, [vp, cf]),
+    "rmd_seeds_propagate_prior": (ci, [vp, vp, cf]),
     "rmd_seeds_update": (ci, [vp, vp, vp]),
     "rmd_seeds_update_u8": (ci, [vp, vp, vp]),
     "rmd_seeds_update_device": (ci, [vp, vp, cs, vp]),

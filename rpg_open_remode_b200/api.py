@@ -46,6 +46,8 @@ OPT_TUNE_CTAS_PER_SM = 19
 OPT_TUNE_WARP_TILE_CANDS = 20
 FIELD_DEBUG_TIMELINE = 100
 VARIANT_STAGED, VARIANT_DIRECT = 0, 1
+# sigma^2 of a propagated keyframe prior as a fraction of the uniform prior's range^2 / 36 (DESIGN.md 4.7, 6)
+PRIOR_SIGMA_SQ_FRAC = 1.0 / 16.0
 
 _f32 = np.float32
 
@@ -367,6 +369,17 @@ class SeedMatrix:
               "SeedMatrix::pointCloud")
         return out[:min(cap, n.value)], int(n.value)
 
+    def setPriorPropagation(self, sigma_sq_frac: float) -> None:
+        """In place: from now on every setReferenceImage* first splats this keyframe's CONVERGED seeds into the new
+        reference view and uses them as its depth prior (sigma^2 = sigma_sq_frac * range^2 / 36).  0 = off."""
+        check(self._L.rmd_seeds_set_prior_propagation(self._h, float(sigma_sq_frac)), "SeedMatrix::setPriorPropagation")
+
+    def propagatePriorFrom(self, src: "SeedMatrix", sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC) -> None:
+        """Right after setReferenceImage* (no update since): take this keyframe's depth prior from the CONVERGED
+        seeds of another live keyframe `src` (same device; size and camera may differ)."""
+        check(self._L.rmd_seeds_propagate_prior(self._h, src.handle, float(sigma_sq_frac)),
+              "SeedMatrix::propagatePriorFrom")
+
     def uploadState(self, field: int, values) -> None:
         dt = np.int32 if field == FIELD_CONVERGENCE else np.float32
         a = np.ascontiguousarray(values, dtype=dt)
@@ -554,6 +567,11 @@ class Depthmap:
         self.ref_img_undistorted_8uc1_ = self.seeds_.undistort(img) if self.is_distorted_ else np.array(img, copy=True)
         self.T_world_ref_ = (T_curr_world if isinstance(T_curr_world, SE3) else SE3(T_curr_world)).inv()
         return ret
+
+    def setPriorPropagation(self, sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC) -> None:
+        """Each new reference frame takes its depth prior from the converged seeds of the keyframe it replaces
+        (SeedMatrix.setPriorPropagation); 0 switches it off (the default of a new Depthmap)."""
+        self.seeds_.setPriorPropagation(sigma_sq_frac)
 
     def update(self, img_curr, T_curr_world) -> None:
         self.seeds_.update(self._input_image(img_curr), T_curr_world)

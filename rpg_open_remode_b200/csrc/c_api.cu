@@ -20,6 +20,7 @@
 #include "host_copy.h"
 #include "ingest.cuh"
 #include "point_cloud.cuh"
+#include "prior.cuh"
 #include "depth_filter.cuh"
 #include "reduction.cuh"
 #include "rmd_common.cuh"
@@ -146,6 +147,7 @@ struct rmd_seeds
   float min_depth, max_depth, avg_depth, depth_range, sigma_sq_max;
   float eta_inlier, eta_outlier, epsilon;
   Pose T_world_ref;
+  Pose T_ref_world;       // the pose given to set_reference (its inverse in floats would not be bit-exact)
   float dist_from_ref;
   bool has_reference;
   uint64_t frame_index;   // number of updates since set_reference
@@ -203,6 +205,10 @@ struct rmd_seeds
   cudaEvent_t ext_ev; bool ext_pending;
   // point-cloud extraction (point_cloud.cuh), allocated on first use
   float4 *pc_points; unsigned int *pc_counts, *pc_total;
+  // keyframe prior (prior.cuh): sigma^2 fraction of the in-place option (0 = off); z-buffer and event are
+  // allocated on first use
+  float prior_frac;
+  unsigned int *prior_z; cudaEvent_t prior_ev;
 };
 
 namespace
@@ -316,6 +322,8 @@ void seeds_free(rmd_seeds *s)
   delete s->maps;
   delete s->copier;
   cudaFree(s->pc_points); cudaFree(s->pc_counts); cudaFree(s->pc_total);
+  cudaFree(s->prior_z);
+  if(s->prior_ev) cudaEventDestroy(s->prior_ev);
   if(s->fan_ev) cudaEventDestroy(s->fan_ev);
   if(s->ext_ev) cudaEventDestroy(s->ext_ev);
   cudaFree(s->ref_u8);
@@ -355,11 +363,60 @@ int wait_external(rmd_seeds *s)
   return 0;
 }
 
+// Keyframe prior, step 1 (prior.cuh), on dst->stream: dst's z-buffer <- src's CONVERGED seeds seen from the
+// new reference pose T_curr_world of dst, within [min_depth, max_depth].  src's seeds, convergence map and
+// T_world_ref are read as they are now (src == dst: the keyframe being left).
+int prior_splat(rmd_seeds *dst, const rmd_seeds *src, const float *T_curr_world, float min_depth, float max_depth)
+{
+  const size_t n = (size_t)dst->width * dst->height;
+  if(!dst->prior_z)
+    RMD_CUDA_TRY(cudaMalloc(&dst->prior_z, sizeof(unsigned int) * n));
+  RMD_CUDA_TRY(cudaMemsetAsync(dst->prior_z, 0xFF, sizeof(unsigned int) * n, dst->stream));
+  PriorSplatParams P;
+  memset(&P, 0, sizeof(P));
+  P.src_width = src->width; P.src_height = src->height;
+  P.conv = src->conv; P.conv_stride = (int)(src->conv_pitch / sizeof(int));
+  P.seed = src->seed; P.seed_stride = src->seed_stride;
+  P.src_cam = src->cam;
+  P.T_world_ref = src->T_world_ref;
+  P.dst_width = dst->width; P.dst_height = dst->height;
+  P.dst_cam = dst->cam;
+  P.T_curr_world = pose_from(T_curr_world);
+  P.min_depth = min_depth; P.max_depth = max_depth;
+  P.zbuf = dst->prior_z;
+  RMD_CUDA_TRY(launch_prior_splat(P, dst->stream));
+  dst->n_total += 1;
+  return 0;
+}
+
+// Keyframe prior, step 2, after dst's seed initialisation: the splatted depths become the prior.
+int prior_apply(rmd_seeds *dst, float frac)
+{
+  PriorApplyParams P;
+  memset(&P, 0, sizeof(P));
+  P.width = dst->width; P.height = dst->height;
+  P.zbuf = dst->prior_z;
+  P.conv = dst->conv; P.conv_stride = (int)(dst->conv_pitch / sizeof(int));
+  P.seed = dst->seed; P.seed_stride = dst->seed_stride;
+  P.sigma_sq = frac * dst->sigma_sq_max;
+  RMD_CUDA_TRY(launch_prior_apply(P, dst->stream));
+  dst->n_total += 1;
+  return 0;
+}
+
 // Run the seed-initialisation kernel on the reference image now in s->ref.
 int finish_set_reference(rmd_seeds *s, const float *T_curr_world, float min_depth, float max_depth)
 {
   {
     const int rc = wait_external(s);
+    if(rc) return rc;
+  }
+  // in-place prior: the keyframe being left is splatted before the initialisation overwrites its seeds and
+  // T_world_ref
+  const bool propagate = s->prior_frac > 0.0f && s->has_reference;
+  if(propagate)
+  {
+    const int rc = prior_splat(s, s, T_curr_world, min_depth, max_depth);
     if(rc) return rc;
   }
   s->min_depth = min_depth;
@@ -371,6 +428,7 @@ int finish_set_reference(rmd_seeds *s, const float *T_curr_world, float min_dept
   s->eta_outlier = 0.05f;
   s->epsilon = s->depth_range / 1000.0f;
   s->T_world_ref = pose_inverse(pose_from(T_curr_world));
+  s->T_ref_world = pose_from(T_curr_world);
 
   InitParams ip;
   ip.width = s->width; ip.height = s->height;
@@ -380,6 +438,11 @@ int finish_set_reference(rmd_seeds *s, const float *T_curr_world, float min_dept
   ip.conv = s->conv; ip.conv_stride = (int)(s->conv_pitch / sizeof(int));
   ip.avg_depth = s->avg_depth; ip.sigma_sq_max = s->sigma_sq_max;
   RMD_CUDA_TRY(launch_seed_init(ip, s->patch, s->stream));
+  if(propagate)
+  {
+    const int rc = prior_apply(s, s->prior_frac);
+    if(rc) return rc;
+  }
   RMD_CUDA_TRY(cudaMemsetAsync(s->counters, 0, 4 * sizeof(unsigned int), s->stream));
   // the first staged frame of a keyframe starts from the full work list; keys hold "no match"
   s->worklist_valid = false;
@@ -1003,6 +1066,51 @@ int rmd_seeds_set_reference_u8(rmd_seeds_t *s, const uint8_t *host_img, const fl
   RMD_CUDA_TRY(u8_frame_to_float(s, s->ref_u8, s->ref_u8_pitch, s->ref, s->ref_pitch, s->stream));
   s->n_total += 1;
   return finish_set_reference(s, T_curr_world, min_depth, max_depth);
+}
+
+int rmd_seeds_set_prior_propagation(rmd_seeds_t *s, float sigma_sq_frac)
+{
+  RMD_REQUIRE(s, "rmd_seeds_set_prior_propagation: null handle");
+  RMD_REQUIRE(sigma_sq_frac >= 0.0f && sigma_sq_frac <= 1.0f,
+              "rmd_seeds_set_prior_propagation: sigma_sq_frac must be in [0, 1] (0 = off)");
+  s->prior_frac = sigma_sq_frac;
+  return 0;
+}
+
+int rmd_seeds_propagate_prior(rmd_seeds_t *dst, const rmd_seeds_t *src, float sigma_sq_frac)
+{
+  RMD_REQUIRE(dst && src, "rmd_seeds_propagate_prior: null handle");
+  RMD_REQUIRE(sigma_sq_frac > 0.0f && sigma_sq_frac <= 1.0f, "rmd_seeds_propagate_prior: sigma_sq_frac must be in (0, 1]");
+  RMD_REQUIRE(dst != src, "rmd_seeds_propagate_prior: src == dst (use rmd_seeds_set_prior_propagation)");
+  RMD_REQUIRE(dst->device == src->device, "rmd_seeds_propagate_prior: handles on different devices");
+  if(!dst->has_reference || dst->frame_index != 0)
+    return fail(RMD_ERR_NOT_INITIALISED,
+                "rmd_seeds_propagate_prior: dst needs a reference frame set since its last update");
+  if(!src->has_reference)
+    return fail(RMD_ERR_NOT_INITIALISED, "rmd_seeds_propagate_prior: src has no reference frame");
+  DeviceGuard guard(dst->device);
+  {
+    const int rc = wait_external(dst);
+    if(rc) return rc;
+  }
+  // The splat runs on dst's stream after everything that writes src's state: src's own stream, and work
+  // another handle enqueued against src's buffers.
+  rmd_seeds *s = const_cast<rmd_seeds*>(src);   // only its ordering book-keeping changes
+  if(!dst->prior_ev)
+    RMD_CUDA_TRY(cudaEventCreateWithFlags(&dst->prior_ev, cudaEventDisableTiming));
+  RMD_CUDA_TRY(cudaEventRecord(dst->prior_ev, s->stream));
+  RMD_CUDA_TRY(cudaStreamWaitEvent(dst->stream, dst->prior_ev, 0));
+  if(s->ext_pending)
+    RMD_CUDA_TRY(cudaStreamWaitEvent(dst->stream, s->ext_ev, 0));
+  {
+    const int rc = prior_splat(dst, s, dst->T_ref_world.m, dst->min_depth, dst->max_depth);
+    if(rc) return rc;
+  }
+  // a later writer of src's seeds (update, set_reference, upload_state) waits for the splat's reads; the wait
+  // above already covers any earlier external event, so re-recording ext_ev loses nothing
+  RMD_CUDA_TRY(cudaEventRecord(s->ext_ev, dst->stream));
+  s->ext_pending = true;
+  return prior_apply(dst, sigma_sq_frac);
 }
 
 int rmd_seeds_update(rmd_seeds_t *s, const float *host_img, const float *T_curr_world)

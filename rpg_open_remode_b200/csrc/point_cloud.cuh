@@ -32,6 +32,28 @@ struct PointCloudParams
 constexpr int POINT_CLOUD_BLOCK = 256;          // threads
 constexpr int POINT_CLOUD_PIXELS = 4 * POINT_CLOUD_BLOCK;   // consecutive pixels (row-major) per block
 
+// World point of pixel (x, y) at distance `depth` along its ray.  IEEE arithmetic in the order of the
+// reference's host code (gcc -O3, no contraction): f = normalize((x-cx)/fx, (y-cy)/fy, 1) with normalize =
+// v * (1 / sqrtf(dot)), xyz = T_world_ref * (f * depth)  (src/publisher.cpp:73-74, helper_math.h:1309-1313,
+// se3.cuh:111-124,165-168).  Shared by the point cloud and the keyframe prior (prior.cuh), whose splat must
+// start from exactly the published points.
+__device__ __forceinline__ float3 back_project(const Camera &cam, const Pose &T_world_ref, int x, int y, float depth)
+{
+  const float vx = __fdiv_rn(__fsub_rn((float)x, cam.cx), cam.fx);
+  const float vy = __fdiv_rn(__fsub_rn((float)y, cam.cy), cam.fy);
+  const float dot = __fadd_rn(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)), 1.0f);   // + 1.0f * 1.0f
+  const float inv_len = __fdiv_rn(1.0f, __fsqrt_rn(dot));
+  const float px = __fmul_rn(__fmul_rn(vx, inv_len), depth);
+  const float py = __fmul_rn(__fmul_rn(vy, inv_len), depth);
+  const float pz = __fmul_rn(__fmul_rn(1.0f, inv_len), depth);
+  const float *T = T_world_ref.m;
+  float3 o;
+  o.x = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], px), __fmul_rn(T[1], py)), __fmul_rn(T[2], pz)), T[3]);
+  o.y = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4], px), __fmul_rn(T[5], py)), __fmul_rn(T[6], pz)), T[7]);
+  o.z = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[8], px), __fmul_rn(T[9], py)), __fmul_rn(T[10], pz)), T[11]);
+  return o;
+}
+
 // Two launches: count (+ scan of the block totals by the last block), write.
 cudaError_t launch_point_cloud(const PointCloudParams &P, cudaStream_t stream);
 

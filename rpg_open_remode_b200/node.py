@@ -17,7 +17,7 @@ from typing import Callable, List, Optional
 
 import numpy as np
 
-from .api import SE3, Depthmap, SeedMatrix
+from .api import PRIOR_SIGMA_SQ_FRAC, SE3, Depthmap, SeedMatrix
 
 UPDATE, TAKE_REFERENCE_FRAME = 0, 1   # rmd::ProcessingStates::State, include/rmd/depthmap_node.h:32-36
 
@@ -76,8 +76,14 @@ class KeyframeSet:
         self.seeds: List[SeedMatrix] = [SeedMatrix(width, height, camera, patch_side, device) for _ in range(n)]
         self.live: List[bool] = [False] * n
 
-    def setReferenceImage(self, slot: int, img, T_curr_world, min_depth: float, max_depth: float) -> None:
+    def setReferenceImage(self, slot: int, img, T_curr_world, min_depth: float, max_depth: float,
+                          prior_from: Optional[int] = None, sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC) -> None:
+        """prior_from: another live slot whose converged seeds become the new keyframe's depth prior."""
+        if prior_from is not None and (prior_from == slot or not self.live[prior_from]):
+            raise ValueError("KeyframeSet.setReferenceImage: prior_from must be another live slot")
         self.seeds[slot].setReferenceImage(img, T_curr_world, min_depth, max_depth)
+        if prior_from is not None:
+            self.seeds[slot].propagatePriorFrom(self.seeds[prior_from], sigma_sq_frac)
         self.live[slot] = True
 
     def retire(self, slot: int) -> None:
