@@ -1,0 +1,98 @@
+// rmd/tsdf_volume.cuh -- rmd::TsdfVolume: fusion of finished keyframes into a dense TSDF voxel grid
+// (DESIGN.md 4.8).  The reference has no such class; this one is a host-only forwarder to the C-ABI
+// (rmd_volume_*, include/rmd_b200.h) that throws rmd::CudaException on failure, like rmd::SeedMatrix.
+#ifndef TSDF_VOLUME_CUH
+#define TSDF_VOLUME_CUH
+
+#include <cstddef>
+#include <vector>
+
+#include <rmd/pinhole_camera.cuh>
+#include <rmd/se3.cuh>
+#include <rmd/seed_matrix.cuh>
+
+namespace rmd
+{
+
+class TsdfVolume
+{
+public:
+  // nx * ny * nz voxels (x fastest) of edge voxel_size; origin = world position of the centre of voxel (0, 0, 0).
+  TsdfVolume(int nx, int ny, int nz, float voxel_size, const float origin[3], float truncation, float max_weight,
+             int device = -1)
+    : handle_(NULL)
+  {
+    detail::throw_on_error(rmd_volume_create(nx, ny, nz, voxel_size, origin, truncation, max_weight, device, &handle_),
+                           "TsdfVolume: unable to create");
+  }
+
+  ~TsdfVolume() { rmd_volume_destroy(handle_); }
+
+  // A finished keyframe: the CONVERGED seeds of `seeds` at the pose their reference was set with; depth = their mu
+  // (dev_depth NULL) or a pitched device image such as rmd::DepthmapDenoiser's output.
+  void integrate(const SeedMatrix &seeds, const float *dev_depth = NULL, size_t depth_pitch = 0)
+  {
+    detail::throw_on_error(rmd_volume_integrate_seeds(handle_, seeds.handle(), dev_depth, depth_pitch),
+                           "TsdfVolume: unable to integrate the keyframe");
+  }
+
+  // Any depth image on the device; dev_conv NULL = every finite positive depth counts.
+  void integrateDepth(int width, int height, const PinholeCamera &cam, const SE3<float> &T_curr_world,
+                      const float *dev_depth, size_t depth_pitch, const int *dev_conv = NULL, size_t conv_pitch = 0)
+  {
+    detail::throw_on_error(rmd_volume_integrate_depth(handle_, width, height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                                      T_curr_world.data.data, dev_depth, depth_pitch, dev_conv,
+                                                      conv_pitch),
+                           "TsdfVolume: unable to integrate the depth image");
+  }
+
+  // (x, y, z, weight) of every surface point, 4 floats per point.
+  std::vector<float> surfacePoints()
+  {
+    size_t n = 0;
+    detail::throw_on_error(rmd_volume_surface_points(handle_, NULL, 0, &n), "TsdfVolume: unable to count points");
+    std::vector<float> out(4 * n);
+    if(n)
+      detail::throw_on_error(rmd_volume_surface_points(handle_, out.data(), n, &n),
+                             "TsdfVolume: unable to extract points");
+    out.resize(4 * n < out.size() ? 4 * n : out.size());
+    return out;
+  }
+
+  // Distance along each pixel's ray to the fused surface (0 = none) into a pitched device image; asynchronous on
+  // the volume's stream (sync() before another stream reads it).
+  void raycast(int width, int height, const PinholeCamera &cam, const SE3<float> &T_curr_world, float *dev_depth,
+               size_t depth_pitch)
+  {
+    detail::throw_on_error(rmd_volume_raycast(handle_, width, height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                              T_curr_world.data.data, dev_depth, depth_pitch),
+                           "TsdfVolume: unable to raycast");
+  }
+
+  void download(float *host_tsdf, float *host_weight)
+  {
+    detail::throw_on_error(rmd_volume_download(handle_, host_tsdf, host_weight), "TsdfVolume: unable to download");
+  }
+  void upload(const float *host_tsdf, const float *host_weight)
+  {
+    detail::throw_on_error(rmd_volume_upload(handle_, host_tsdf, host_weight), "TsdfVolume: unable to upload");
+  }
+  void reset() { detail::throw_on_error(rmd_volume_reset(handle_), "TsdfVolume: unable to reset"); }
+  void setStream(cudaStream_t stream)
+  {
+    detail::throw_on_error(rmd_volume_set_stream(handle_, stream), "TsdfVolume: unable to set the stream");
+  }
+  void sync() { detail::throw_on_error(rmd_volume_sync(handle_), "TsdfVolume: unable to synchronise"); }
+
+  rmd_volume_t *handle() const { return handle_; }
+
+private:
+  TsdfVolume(const TsdfVolume &);
+  TsdfVolume &operator=(const TsdfVolume &);
+
+  rmd_volume_t *handle_;
+};
+
+} // rmd namespace
+
+#endif // TSDF_VOLUME_CUH

@@ -131,6 +131,7 @@ enum rmd_seeds_option {
 typedef struct rmd_seeds rmd_seeds_t;
 typedef struct rmd_denoiser rmd_denoiser_t;
 typedef struct rmd_multi rmd_multi_t;
+typedef struct rmd_volume rmd_volume_t;
 
 /* ------------------------------------------------------------------ misc */
 int rmd_abi_version(void);
@@ -393,6 +394,92 @@ int rmd_multi_size(rmd_multi_t *m, int *n_ranks, int *n_local, int *first_rank);
 int rmd_multi_gather_maps(rmd_multi_t *m, rmd_seeds_t *const *seeds,
                           const float *const *dev_depth, const size_t *dev_depth_pitch,
                           int root, float *host_depth, int32_t *host_conv);
+
+/* ------------------------------------------------------------ TSDF volume */
+
+/* Fusion of finished keyframes into one dense truncated signed distance
+ * function on the device (DESIGN.md 4.8; the reference publishes every
+ * keyframe's point cloud on its own and leaves fusion to the consumer).
+ * Voxel (i, j, k), 0 <= i < nx (x fastest), holds (tsdf, weight); its world
+ * position is origin + (i, j, k) * voxel_size, so origin is the CENTRE of
+ * voxel (0, 0, 0).  Weight 0 = unknown.  All arithmetic is IEEE
+ * round-to-nearest in a fixed operation order (bit-reproducible).
+ *
+ * A new volume is all unknown.  truncation tau (metres) > 0; max_weight >= 1
+ * caps the weight of a voxel (one observation = 1).  At most 2^31 voxels.
+ * device < 0: current.  Returns RMD_ERR_INVALID_ARGUMENT for a null pointer,
+ * a dimension <= 0, too many voxels, voxel_size or truncation <= 0, or
+ * max_weight < 1. */
+int rmd_volume_create(int nx, int ny, int nz, float voxel_size, const float origin[3], float truncation,
+                      float max_weight, int device, rmd_volume_t **out);
+int rmd_volume_destroy(rmd_volume_t *v);
+/* Run this volume's work on a caller-owned cudaStream_t (NULL = its own). */
+int rmd_volume_set_stream(rmd_volume_t *v, void *cuda_stream);
+/* Every voxel back to (0, 0), asynchronously on the volume's stream. */
+int rmd_volume_reset(rmd_volume_t *v);
+int rmd_volume_sync(rmd_volume_t *v);
+/* Any output pointer may be NULL. */
+int rmd_volume_size(rmd_volume_t *v, int *nx, int *ny, int *nz, float *voxel_size, float origin[3]);
+
+/* Integrate one keyframe: every voxel in front of the camera whose projection
+ * u = floor(fx x / z + cx + 0.5), v = floor(fy y / z + cy + 0.5) lies in the
+ * image, on a CONVERGED pixel with a finite depth d > 0, and not more than tau
+ * behind the surface (sdf = d - |p| >= -tau, p in camera coordinates), gets
+ * the observation o = min(1, sdf / tau):  w' = w + 1,  t' = (t w + o) / w',
+ * stored as (t', min(w', max_weight)).  Voxels in front of the surface get
+ * o = 1 (free space carves out earlier outliers); all others are untouched.
+ *
+ * The keyframe is s: its camera, the pose it was set with and its
+ * convergence map.  Depth (distance along the ray) is the seeds' mu when
+ * dev_depth is NULL, else a pitched device image of s's size (pitch in bytes,
+ * >= width * 4 and a multiple of 4), e.g. the output of
+ * rmd_denoiser_run_seeds_to_device.  Asynchronous on the volume's stream,
+ * ordered on the device like rmd_seeds_propagate_prior with its source: the
+ * integration waits for s's queued work and for a denoised image pending
+ * against s, and a later update / set_reference / upload_state of s waits
+ * for the integration.  RMD_ERR_INVALID_ARGUMENT: null handle, bad pitch,
+ * volume and seeds on different devices.  RMD_ERR_NOT_INITIALISED: s has no
+ * reference frame. */
+int rmd_volume_integrate_seeds(rmd_volume_t *v, rmd_seeds_t *s, const float *dev_depth, size_t depth_pitch);
+/* Same for any depth image already on the device, seen by the pinhole camera
+ * (fx, fy, cx, cy) at T_curr_world (world -> camera).  dev_conv: int32
+ * states (pitch in bytes), only CONVERGED pixels count; NULL = every pixel
+ * with a finite positive depth counts.  Asynchronous on the volume's stream:
+ * the images must be complete when it runs (produced on that stream or
+ * synchronised).  RMD_ERR_INVALID_ARGUMENT: null pointer, size <= 0, pitch
+ * smaller than a row or not a multiple of 4. */
+int rmd_volume_integrate_depth(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                               const float *T_curr_world, const float *dev_depth, size_t depth_pitch,
+                               const int32_t *dev_conv, size_t conv_pitch);
+
+/* The surface as points.  For each voxel a and each of its +x, +y, +z
+ * neighbours b inside the grid: a point when both weights are > 0, both
+ * |tsdf| < 1 and the signs differ (t_a > 0 >= t_b or t_a <= 0 < t_b), at
+ * p_a + t_a / (t_a - t_b) * voxel_size along that axis, with
+ * w = min(w_a, w_b).  4 floats (x, y, z, w) per point, ordered by voxel index,
+ * then axis x, y, z.  *count is always the number of points; at most
+ * `capacity` are written.  The host variant stages min(count, capacity)
+ * points in device memory it keeps (grown on demand).  Synchronous. */
+int rmd_volume_surface_points(rmd_volume_t *v, float *host_xyzw, size_t capacity, size_t *count);
+/* Same into device memory (16-byte aligned). */
+int rmd_volume_surface_points_device(rmd_volume_t *v, float *dev_xyzw, size_t capacity, size_t *count);
+
+/* Depth map of the fused surface seen by the pinhole camera (fx, fy, cx, cy)
+ * at T_curr_world: the ray of pixel (x, y), normalize((x-cx)/fx, (y-cy)/fy,
+ * 1) rotated into the world from the camera centre, is clipped to the box of
+ * the voxel centres and sampled every voxel_size with trilinear
+ * interpolation; a sample with a corner outside the grid or unknown is
+ * unknown.  The first pair of consecutive known samples f_prev > 0 >= f gives
+ * the distance along the ray  t_prev + s f_prev / (f_prev - f);  0 where there
+ * is none.  dev_depth: pitched float image (pitch in bytes).  Asynchronous on
+ * the volume's stream (rmd_volume_sync before another stream reads it). */
+int rmd_volume_raycast(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                       const float *T_curr_world, float *dev_depth, size_t depth_pitch);
+
+/* Test / checkpoint hooks (like rmd_seeds_upload_state): nx * ny * nz floats
+ * each, x fastest.  Synchronous. */
+int rmd_volume_download(rmd_volume_t *v, float *host_tsdf, float *host_weight);
+int rmd_volume_upload(rmd_volume_t *v, const float *host_tsdf, const float *host_weight);
 
 /* ---------------------------------------------------------- device image */
 

@@ -71,7 +71,20 @@ _SIGNATURES = {
     "rmd_multi_destroy": (ci, [vp]),
     "rmd_multi_size": (ci, [vp, P(ci), P(ci), P(ci)]),
     "rmd_multi_gather_maps": (ci, [vp, P(vp), P(vp), P(cs), ci, vp, vp]),
-    "rmd_reduce_sum_f32": (ci, [vp, cs, cs, cs, P(cf)]),
+    "rmd_volume_create": (ci, [ci, ci, ci, cf, vp, cf, cf, ci, P(vp)]),
+    "rmd_volume_destroy": (ci, [vp]),
+    "rmd_volume_set_stream": (ci, [vp, vp]),
+    "rmd_volume_reset": (ci, [vp]),
+    "rmd_volume_sync": (ci, [vp]),
+    "rmd_volume_size": (ci, [vp, P(ci), P(ci), P(ci), P(cf), vp]),
+    "rmd_volume_integrate_seeds": (ci, [vp, vp, vp, cs]),
+    "rmd_volume_integrate_depth": (ci, [vp, ci, ci, cf, cf, cf, cf, vp, vp, cs, vp, cs]),
+    "rmd_volume_surface_points": (ci, [vp, vp, cs, P(cs)]),
+    "rmd_volume_surface_points_device": (ci, [vp, vp, cs, P(cs)]),
+    "rmd_volume_raycast": (ci, [vp, ci, ci, cf, cf, cf, cf, vp, vp, cs]),
+    "rmd_volume_download": (ci, [vp, vp, vp]),
+    "rmd_volume_upload": (ci, [vp, vp, vp]),
+    "rmd_reduce_sum_f32":(ci, [vp, cs, cs, cs, P(cf)]),
     "rmd_reduce_sum_i32": (ci, [vp, cs, cs, cs, P(ctypes.c_int32)]),
     "rmd_reduce_count_eq_i32": (ci, [vp, cs, cs, cs, ctypes.c_int32, P(cs)]),
     "rmd_reduce_min_max_f32": (ci, [vp, cs, cs, cs, P(cf), P(cf)]),

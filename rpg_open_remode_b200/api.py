@@ -501,6 +501,109 @@ class DepthmapDenoiser:
         return int(n.value)
 
 
+class TsdfVolume:
+    """Dense TSDF voxel grid on one device that fuses finished keyframes (rmd_volume_*, include/rmd_b200.h;
+    DESIGN.md 4.8).  dims = (nx, ny, nz), x fastest; origin = world position of the centre of voxel (0, 0, 0);
+    truncation in metres; max_weight caps a voxel's weight (one observation = 1)."""
+
+    def __init__(self, dims, voxel_size: float, origin, truncation: float, max_weight: float = 64.0, device=-1):
+        self.dims = tuple(int(n) for n in dims)
+        if len(self.dims) != 3:
+            raise ValueError("TsdfVolume: dims must be (nx, ny, nz)")
+        self._L = _native.lib()
+        o = np.ascontiguousarray(np.asarray(origin, _f32).reshape(3))
+        h = ctypes.c_void_p()
+        check(self._L.rmd_volume_create(*self.dims, float(voxel_size), o.ctypes.data, float(truncation),
+                                        float(max_weight), int(device), ctypes.byref(h)), "TsdfVolume")
+        self._h = h
+        self.voxel_size, self.origin = float(_f32(voxel_size)), o.copy()
+        self.truncation, self.max_weight = float(_f32(truncation)), float(_f32(max_weight))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            self._L.rmd_volume_destroy(h)
+
+    @property
+    def handle(self):
+        return self._h
+
+    def integrate(self, seeds: SeedMatrix, depth: "DeviceImage | None" = None) -> None:
+        """A keyframe: the CONVERGED pixels of `seeds`, seen from the pose its reference was set with; depth = the
+        seeds' mu or a device image of their size (e.g. denoised).  Ordered on the device against `seeds`."""
+        ptr, pitch = (depth.data, depth.pitch) if depth is not None else (None, 0)
+        check(self._L.rmd_volume_integrate_seeds(self._h, seeds.handle, ptr, pitch), "TsdfVolume::integrate")
+
+    def integrateDepth(self, depth, cam: PinholeCamera, T_curr_world, conv=None) -> None:
+        """Any depth image (distance along the ray): a float32 DeviceImage or a host array; conv: optional int32
+        states (DeviceImage or host array), only CONVERGED pixels count."""
+        keep = []
+
+        def dev(img, dtype):
+            if isinstance(img, DeviceImage):
+                return img
+            a = np.ascontiguousarray(img, dtype)
+            d = DeviceImage(a.shape[1], a.shape[0], dtype)
+            d.setDevData(a)
+            keep.append(d)
+            return d
+
+        D = dev(depth, np.float32)
+        C = dev(conv, np.int32) if conv is not None else None
+        if C is not None and (C.width, C.height) != (D.width, D.height):
+            raise ValueError("TsdfVolume::integrateDepth: depth and state maps differ in size")
+        T = _pose12(T_curr_world)
+        check(self._L.rmd_volume_integrate_depth(self._h, D.width, D.height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                                 T.ctypes.data, D.data, D.pitch, C.data if C else None,
+                                                 C.pitch if C else 0), "TsdfVolume::integrateDepth")
+        if keep:
+            self.sync()   # the staged images must outlive the kernel
+
+    def surfacePoints(self, capacity: "int | None" = None) -> np.ndarray:
+        """float32 [n, 4] = (x, y, z, weight) of the zero crossings, in voxel order then axis x, y, z.  With a
+        capacity, at most that many points."""
+        n = ctypes.c_size_t()
+        if capacity is None:
+            check(self._L.rmd_volume_surface_points(self._h, None, 0, ctypes.byref(n)), "TsdfVolume::surfacePoints")
+            capacity = n.value
+        out = np.empty((int(capacity), 4), np.float32)
+        check(self._L.rmd_volume_surface_points(self._h, out.ctypes.data if capacity else None, int(capacity),
+                                                ctypes.byref(n)), "TsdfVolume::surfacePoints")
+        return out[:min(int(capacity), n.value)]
+
+    def raycast(self, cam: PinholeCamera, T_curr_world, width: int, height: int) -> np.ndarray:
+        """float32 [height, width]: distance along each pixel's ray to the fused surface, 0 where none."""
+        img = DeviceImage(width, height, "float32")
+        T = _pose12(T_curr_world)
+        check(self._L.rmd_volume_raycast(self._h, int(width), int(height), cam.fx, cam.fy, cam.cx, cam.cy,
+                                         T.ctypes.data, img.data, img.pitch), "TsdfVolume::raycast")
+        self.sync()
+        return img.getDevData()
+
+    def download(self):
+        """(tsdf, weight), float32 arrays of shape (nz, ny, nx)."""
+        nx, ny, nz = self.dims
+        t, w = np.empty((nz, ny, nx), np.float32), np.empty((nz, ny, nx), np.float32)
+        check(self._L.rmd_volume_download(self._h, t.ctypes.data, w.ctypes.data), "TsdfVolume::download")
+        return t, w
+
+    def upload(self, tsdf, weight) -> None:
+        nx, ny, nz = self.dims
+        t, w = (np.ascontiguousarray(a, np.float32) for a in (tsdf, weight))
+        if t.size != nx * ny * nz or w.size != nx * ny * nz:
+            raise ValueError("TsdfVolume::upload: wrong size")
+        check(self._L.rmd_volume_upload(self._h, t.ctypes.data, w.ctypes.data), "TsdfVolume::upload")
+
+    def reset(self) -> None:
+        check(self._L.rmd_volume_reset(self._h), "TsdfVolume::reset")
+
+    def setStream(self, cuda_stream: int) -> None:
+        check(self._L.rmd_volume_set_stream(self._h, cuda_stream), "TsdfVolume::setStream")
+
+    def sync(self) -> None:
+        check(self._L.rmd_volume_sync(self._h), "TsdfVolume::sync")
+
+
 class ImageReducer:
     """rmd::ImageReducer<T> -- include/rmd/reduction.cuh:27-62.  The launch
     shape arguments of the reference are accepted and ignored (the kernel
@@ -553,6 +656,7 @@ class Depthmap:
         self.ref_img_undistorted_8uc1_ = np.zeros((height, width), np.uint8)
         self.T_world_ref_ = SE3()
         self.is_distorted_ = False
+        self.denoised_dev_ = None   # device copy of the denoised map for fuseDenoisedInto, allocated on first use
 
     def initUndistortionMap(self, k1, k2, r1, r2):
         """src/depthmap.cpp:45-61; the maps and the per-frame remap live on the GPU."""
@@ -581,6 +685,17 @@ class Depthmap:
 
     def downloadDenoisedDepthmap(self, lam, iterations) -> None:
         self.output_depth_32fc1_ = self.denoiser_.denoiseSeeds(self.seeds_, lam, iterations)
+
+    def fuseDenoisedInto(self, volume: TsdfVolume, lam, iterations) -> None:
+        """downloadDenoisedDepthmap (the same host map, bit for bit) and the keyframe's integration into `volume`
+        from the denoised device image, masked by the CONVERGED seeds: one denoiser run for both."""
+        if self.denoised_dev_ is None:
+            self.denoised_dev_ = DeviceImage(self.width_, self.height_, "float32")
+        img = self.denoised_dev_
+        self.denoiser_.denoiseSeedsToDevice(self.seeds_, img.data, img.pitch, lam, iterations)
+        self.denoiser_.sync()
+        self.output_depth_32fc1_ = img.getDevData()
+        volume.integrate(self.seeds_, img)
 
     def getDepthmap(self):
         return self.output_depth_32fc1_

@@ -25,6 +25,7 @@
 #include "reduction.cuh"
 #include "rmd_common.cuh"
 #include "staged_maps.cuh"
+#include "volume.cuh"
 
 namespace rmdb
 {
@@ -2071,6 +2072,333 @@ int rmd_image_copy(void *dst, size_t dst_pitch, const void *src, size_t src_pitc
   RMD_REQUIRE(dst && src, "rmd_image_copy: null argument");
   RMD_CUDA_TRY(cudaMemcpy2D(dst, dst_pitch, src, src_pitch, width * elem_size, height,
                             cudaMemcpyDeviceToDevice));
+  return 0;
+}
+
+} // extern "C"
+
+// ============================================================ TSDF volume
+
+struct rmd_volume
+{
+  int device;
+  VolumeGrid g;               // g.vox: nx * ny * nz float2 (tsdf, weight)
+  size_t n_vox;
+  float trunc, max_weight;
+  cudaStream_t own_stream, stream;
+  cudaEvent_t seeds_ev;       // integrate_seeds: the seeds' stream has produced what the kernel reads
+  // surface points (allocated on first use): per-block offsets, total, host staging grown on demand
+  unsigned long long *surf_offsets, *surf_total;
+  float4 *stage; size_t stage_cap;
+  uint64_t n_total;
+};
+
+namespace
+{
+
+const size_t kVolumeMaxVoxels = (size_t)1 << 31;
+const size_t kVolumeChunk = (size_t)1 << 24;   // voxels per host staging chunk of download / upload
+
+bool depth_pitch_ok(size_t pitch, int width)
+{
+  return pitch >= sizeof(float) * (size_t)width && pitch % sizeof(float) == 0;
+}
+
+int volume_integrate(rmd_volume *v, int width, int height, const Camera &cam, const Pose &T_curr_world,
+                     const float *depth, size_t depth_stride, int depth_comps, const int32_t *conv, size_t conv_stride)
+{
+  VolumeIntegrateParams P;
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.width = width; P.height = height;
+  P.cam = cam;
+  P.T_curr_world = T_curr_world;
+  P.depth = depth; P.depth_stride = depth_stride; P.depth_comps = depth_comps;
+  P.conv = conv; P.conv_stride = conv_stride;
+  P.trunc = v->trunc; P.max_weight = v->max_weight;
+  RMD_CUDA_TRY(launch_volume_integrate(P, v->stream));
+  v->n_total += 1;
+  return 0;
+}
+
+// Count pass + scan: returns the number of surface points (synchronises the volume's stream).
+int volume_surface_count(rmd_volume *v, VolumeSurfaceParams &P, size_t *count)
+{
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.n_blocks = (unsigned int)((v->n_vox + VOLUME_SURF_VOXELS - 1) / VOLUME_SURF_VOXELS);
+  if(!v->surf_offsets)
+  {
+    RMD_CUDA_TRY(cudaMalloc(&v->surf_offsets, sizeof(unsigned long long) * P.n_blocks));
+    RMD_CUDA_TRY(cudaMalloc(&v->surf_total, sizeof(unsigned long long)));
+  }
+  P.block_offsets = v->surf_offsets;
+  P.total = v->surf_total;
+  RMD_CUDA_TRY(launch_volume_surface_count(P, v->stream));
+  v->n_total += 2;
+  unsigned long long n = 0;
+  RMD_CUDA_TRY(cudaMemcpyAsync(&n, v->surf_total, sizeof(n), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  *count = (size_t)n;
+  return 0;
+}
+
+int volume_surface_write(rmd_volume *v, VolumeSurfaceParams &P, float4 *out, size_t capacity)
+{
+  P.out = out;
+  P.capacity = capacity;
+  RMD_CUDA_TRY(launch_volume_surface_write(P, v->stream));
+  v->n_total += 1;
+  return 0;
+}
+
+} // namespace
+
+extern "C"
+{
+
+int rmd_volume_create(int nx, int ny, int nz, float voxel_size, const float origin[3], float truncation,
+                      float max_weight, int device, rmd_volume_t **out)
+{
+  RMD_REQUIRE(out, "rmd_volume_create: out is null");
+  *out = NULL;
+  RMD_REQUIRE(origin, "rmd_volume_create: origin is null");
+  RMD_REQUIRE(nx > 0 && ny > 0 && nz > 0, "rmd_volume_create: grid dimensions must be positive");
+  const uint64_t plane = (uint64_t)nx * (uint64_t)ny;   // each factor < 2^31: no overflow in 64 bits
+  RMD_REQUIRE(plane <= kVolumeMaxVoxels && plane * (uint64_t)nz <= kVolumeMaxVoxels,
+              "rmd_volume_create: at most 2^31 voxels");
+  RMD_REQUIRE(voxel_size > 0.0f && isfinite(voxel_size), "rmd_volume_create: voxel_size must be > 0");
+  RMD_REQUIRE(truncation > 0.0f && isfinite(truncation), "rmd_volume_create: truncation must be > 0");
+  RMD_REQUIRE(max_weight >= 1.0f, "rmd_volume_create: max_weight must be >= 1");
+  RMD_REQUIRE(isfinite(origin[0]) && isfinite(origin[1]) && isfinite(origin[2]), "rmd_volume_create: bad origin");
+  if(device < 0) RMD_CUDA_TRY(cudaGetDevice(&device));
+  DeviceGuard guard(device);
+  rmd_volume *v = new(std::nothrow) rmd_volume();
+  if(!v) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_create: host allocation failed");
+  memset(v, 0, sizeof(*v));
+  v->device = device;
+  v->g.nx = nx; v->g.ny = ny; v->g.nz = nz;
+  v->g.voxel = voxel_size;
+  v->g.ox = origin[0]; v->g.oy = origin[1]; v->g.oz = origin[2];
+  v->n_vox = (size_t)(plane * (uint64_t)nz);
+  v->trunc = truncation; v->max_weight = max_weight;
+  cudaError_t err = cudaStreamCreateWithFlags(&v->own_stream, cudaStreamNonBlocking);
+  if(err == cudaSuccess) err = cudaEventCreateWithFlags(&v->seeds_ev, cudaEventDisableTiming);
+  if(err == cudaSuccess) err = cudaMalloc(&v->g.vox, sizeof(float2) * v->n_vox);
+  if(err == cudaSuccess) err = cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->own_stream);
+  if(err == cudaSuccess) err = cudaStreamSynchronize(v->own_stream);
+  if(err != cudaSuccess)
+  {
+    rmd_volume_destroy(v);
+    return fail_cuda(err, "rmd_volume_create");
+  }
+  v->stream = v->own_stream;
+  *out = v;
+  return 0;
+}
+
+int rmd_volume_destroy(rmd_volume_t *v)
+{
+  if(!v) return 0;
+  DeviceGuard guard(v->device);
+  cudaDeviceSynchronize();
+  if(v->own_stream) cudaStreamDestroy(v->own_stream);
+  if(v->seeds_ev) cudaEventDestroy(v->seeds_ev);
+  cudaFree(v->g.vox);
+  cudaFree(v->surf_offsets); cudaFree(v->surf_total); cudaFree(v->stage);
+  cudaGetLastError();
+  delete v;
+  return 0;
+}
+
+int rmd_volume_set_stream(rmd_volume_t *v, void *cuda_stream)
+{
+  RMD_REQUIRE(v, "rmd_volume_set_stream: null handle");
+  DeviceGuard guard(v->device);
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  v->stream = cuda_stream ? (cudaStream_t)cuda_stream : v->own_stream;
+  return 0;
+}
+
+int rmd_volume_reset(rmd_volume_t *v)
+{
+  RMD_REQUIRE(v, "rmd_volume_reset: null handle");
+  DeviceGuard guard(v->device);
+  RMD_CUDA_TRY(cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->stream));
+  return 0;
+}
+
+int rmd_volume_sync(rmd_volume_t *v)
+{
+  RMD_REQUIRE(v, "rmd_volume_sync: null handle");
+  DeviceGuard guard(v->device);
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  return 0;
+}
+
+int rmd_volume_size(rmd_volume_t *v, int *nx, int *ny, int *nz, float *voxel_size, float origin[3])
+{
+  RMD_REQUIRE(v, "rmd_volume_size: null handle");
+  if(nx) *nx = v->g.nx;
+  if(ny) *ny = v->g.ny;
+  if(nz) *nz = v->g.nz;
+  if(voxel_size) *voxel_size = v->g.voxel;
+  if(origin) { origin[0] = v->g.ox; origin[1] = v->g.oy; origin[2] = v->g.oz; }
+  return 0;
+}
+
+int rmd_volume_integrate_seeds(rmd_volume_t *v, rmd_seeds_t *s, const float *dev_depth, size_t depth_pitch)
+{
+  RMD_REQUIRE(v && s, "rmd_volume_integrate_seeds: null handle");
+  RMD_REQUIRE(v->device == s->device, "rmd_volume_integrate_seeds: volume and seeds on different devices");
+  RMD_REQUIRE(!dev_depth || depth_pitch_ok(depth_pitch, s->width), "rmd_volume_integrate_seeds: bad depth pitch");
+  if(!s->has_reference)
+    return fail(RMD_ERR_NOT_INITIALISED, "rmd_volume_integrate_seeds: the seeds have no reference frame");
+  DeviceGuard guard(v->device);
+  // As rmd_seeds_propagate_prior with its source: run after everything that writes the seeds' state (their own
+  // stream, and work another handle enqueued against them, e.g. the denoised image) ...
+  RMD_CUDA_TRY(cudaEventRecord(v->seeds_ev, s->stream));
+  RMD_CUDA_TRY(cudaStreamWaitEvent(v->stream, v->seeds_ev, 0));
+  if(s->ext_pending)
+    RMD_CUDA_TRY(cudaStreamWaitEvent(v->stream, s->ext_ev, 0));
+  const int rc = dev_depth
+      ? volume_integrate(v, s->width, s->height, s->cam, s->T_ref_world, dev_depth, depth_pitch / sizeof(float), 1,
+                         s->conv, s->conv_pitch / sizeof(int))
+      : volume_integrate(v, s->width, s->height, s->cam, s->T_ref_world, reinterpret_cast<const float*>(s->seed),
+                         (size_t)s->seed_stride * 4, 4, s->conv, s->conv_pitch / sizeof(int));
+  if(rc) return rc;
+  // ... and a later writer of the seeds (update, set_reference, upload_state) waits for the kernel's reads
+  RMD_CUDA_TRY(cudaEventRecord(s->ext_ev, v->stream));
+  s->ext_pending = true;
+  return 0;
+}
+
+int rmd_volume_integrate_depth(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                               const float *T_curr_world, const float *dev_depth, size_t depth_pitch,
+                               const int32_t *dev_conv, size_t conv_pitch)
+{
+  RMD_REQUIRE(v && T_curr_world && dev_depth, "rmd_volume_integrate_depth: null argument");
+  RMD_REQUIRE(width > 0 && height > 0, "rmd_volume_integrate_depth: bad image size");
+  RMD_REQUIRE(depth_pitch_ok(depth_pitch, width), "rmd_volume_integrate_depth: bad depth pitch");
+  RMD_REQUIRE(!dev_conv || (conv_pitch >= sizeof(int32_t) * (size_t)width && conv_pitch % sizeof(int32_t) == 0),
+              "rmd_volume_integrate_depth: bad state pitch");
+  DeviceGuard guard(v->device);
+  Camera cam;
+  cam.fx = fx; cam.fy = fy; cam.cx = cx; cam.cy = cy;
+  return volume_integrate(v, width, height, cam, pose_from(T_curr_world), dev_depth, depth_pitch / sizeof(float), 1,
+                          dev_conv, conv_pitch / sizeof(int32_t));
+}
+
+int rmd_volume_surface_points(rmd_volume_t *v, float *host_xyzw, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (host_xyzw || capacity == 0), "rmd_volume_surface_points: null argument");
+  DeviceGuard guard(v->device);
+  VolumeSurfaceParams P;
+  {
+    const int rc = volume_surface_count(v, P, count);
+    if(rc) return rc;
+  }
+  const size_t n = *count < capacity ? *count : capacity;
+  if(!n)
+    return 0;
+  if(n > v->stage_cap)
+  {
+    RMD_CUDA_TRY(cudaFree(v->stage));
+    v->stage = NULL; v->stage_cap = 0;
+    RMD_CUDA_TRY(cudaMalloc(&v->stage, sizeof(float4) * n));
+    v->stage_cap = n;
+  }
+  {
+    const int rc = volume_surface_write(v, P, v->stage, n);
+    if(rc) return rc;
+  }
+  RMD_CUDA_TRY(cudaMemcpyAsync(host_xyzw, v->stage, n * sizeof(float4), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  return 0;
+}
+
+int rmd_volume_surface_points_device(rmd_volume_t *v, float *dev_xyzw, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (dev_xyzw || capacity == 0), "rmd_volume_surface_points_device: null argument");
+  RMD_REQUIRE(((uintptr_t)dev_xyzw % 16) == 0, "rmd_volume_surface_points_device: output must be 16-byte aligned");
+  DeviceGuard guard(v->device);
+  VolumeSurfaceParams P;
+  {
+    const int rc = volume_surface_count(v, P, count);
+    if(rc) return rc;
+  }
+  const size_t n = *count < capacity ? *count : capacity;
+  if(!n)
+    return 0;
+  {
+    const int rc = volume_surface_write(v, P, reinterpret_cast<float4*>(dev_xyzw), n);
+    if(rc) return rc;
+  }
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  return 0;
+}
+
+int rmd_volume_raycast(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                       const float *T_curr_world, float *dev_depth, size_t depth_pitch)
+{
+  RMD_REQUIRE(v && T_curr_world && dev_depth, "rmd_volume_raycast: null argument");
+  RMD_REQUIRE(width > 0 && height > 0, "rmd_volume_raycast: bad image size");
+  RMD_REQUIRE(depth_pitch_ok(depth_pitch, width), "rmd_volume_raycast: bad depth pitch");
+  DeviceGuard guard(v->device);
+  VolumeRaycastParams P;
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.width = width; P.height = height;
+  P.cam.fx = fx; P.cam.fy = fy; P.cam.cx = cx; P.cam.cy = cy;
+  P.T_world_curr = pose_inverse(pose_from(T_curr_world));
+  P.depth = dev_depth; P.depth_stride = depth_pitch / sizeof(float);
+  RMD_CUDA_TRY(launch_volume_raycast(P, v->stream));
+  v->n_total += 1;
+  return 0;
+}
+
+int rmd_volume_download(rmd_volume_t *v, float *host_tsdf, float *host_weight)
+{
+  RMD_REQUIRE(v && host_tsdf && host_weight, "rmd_volume_download: null argument");
+  DeviceGuard guard(v->device);
+  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
+  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
+  if(!tmp) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_download: host allocation failed");
+  cudaError_t err = cudaSuccess;
+  for(size_t b = 0; b < v->n_vox && err == cudaSuccess; b += chunk)
+  {
+    const size_t m = v->n_vox - b < chunk ? v->n_vox - b : chunk;
+    err = cudaMemcpyAsync(tmp, v->g.vox + b, sizeof(float2) * m, cudaMemcpyDeviceToHost, v->stream);
+    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);
+    for(size_t q = 0; q < m && err == cudaSuccess; ++q)
+    {
+      host_tsdf[b + q] = tmp[q].x;
+      host_weight[b + q] = tmp[q].y;
+    }
+  }
+  free(tmp);
+  RMD_CUDA_TRY(err);
+  return 0;
+}
+
+int rmd_volume_upload(rmd_volume_t *v, const float *host_tsdf, const float *host_weight)
+{
+  RMD_REQUIRE(v && host_tsdf && host_weight, "rmd_volume_upload: null argument");
+  DeviceGuard guard(v->device);
+  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
+  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
+  if(!tmp) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_upload: host allocation failed");
+  cudaError_t err = cudaSuccess;
+  for(size_t b = 0; b < v->n_vox && err == cudaSuccess; b += chunk)
+  {
+    const size_t m = v->n_vox - b < chunk ? v->n_vox - b : chunk;
+    for(size_t q = 0; q < m; ++q)
+      tmp[q] = make_float2(host_tsdf[b + q], host_weight[b + q]);
+    err = cudaMemcpyAsync(v->g.vox + b, tmp, sizeof(float2) * m, cudaMemcpyHostToDevice, v->stream);
+    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);   // tmp is refilled next
+  }
+  free(tmp);
+  RMD_CUDA_TRY(err);
   return 0;
 }
 

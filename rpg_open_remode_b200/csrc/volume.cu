@@ -1,0 +1,391 @@
+// volume.cu -- see volume.cuh.  Integration and extraction stream the voxel records once (HBM-bound); the
+// raycast reads the few voxels around each ray through the read-only path.
+#include "volume.cuh"
+
+namespace rmdb
+{
+
+namespace
+{
+
+__device__ __forceinline__ float voxel_coord(float origin, int i, float s)
+{
+  return __fadd_rn(origin, __fmul_rn((float)i, s));
+}
+
+// One thread per voxel, x fastest, so that the float2 records of a warp are contiguous.  The frustum and depth
+// tests come before the record is loaded: a voxel outside the image costs no memory traffic.
+__global__ void __launch_bounds__(256) volume_integrate_kernel(const VolumeIntegrateParams P)
+{
+  const VolumeGrid &g = P.g;
+  const unsigned int plane = (unsigned int)g.nx * (unsigned int)g.ny;
+  const unsigned int n = blockIdx.x * blockDim.x + threadIdx.x;   // < 2^31 voxels: fits
+  if(n >= plane * (unsigned int)g.nz)
+    return;
+  const int k = (int)(n / plane);
+  const unsigned int rem = n - (unsigned int)k * plane;
+  const int j = (int)(rem / (unsigned int)g.nx);
+  const int i = (int)(rem - (unsigned int)j * (unsigned int)g.nx);
+  const float wx = voxel_coord(g.ox, i, g.voxel), wy = voxel_coord(g.oy, j, g.voxel), wz = voxel_coord(g.oz, k, g.voxel);
+  // p = T_curr_world * w: rotation, then translation (as prior_splat_kernel)
+  const float *T = P.T_curr_world.m;
+  const float px = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[0], wx), __fmul_rn(T[1], wy)), __fmul_rn(T[2], wz)), T[3]);
+  const float py = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4], wx), __fmul_rn(T[5], wy)), __fmul_rn(T[6], wz)), T[7]);
+  const float pz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[8], wx), __fmul_rn(T[9], wy)), __fmul_rn(T[10], wz)), T[11]);
+  if(!(pz > 0.0f))
+    return;
+  const float u = __fadd_rn(__fdiv_rn(__fmul_rn(P.cam.fx, px), pz), P.cam.cx);
+  const float v = __fadd_rn(__fdiv_rn(__fmul_rn(P.cam.fy, py), pz), P.cam.cy);
+  const float tu = floorf(__fadd_rn(u, 0.5f)), tv = floorf(__fadd_rn(v, 0.5f));   // the splat's rounding
+  if(!(tu >= 0.0f && tu < (float)P.width && tv >= 0.0f && tv < (float)P.height))
+    return;
+  const int x = (int)tu, y = (int)tv;
+  if(P.conv && P.conv[(size_t)y * P.conv_stride + x] != RMD_CONVERGED)
+    return;
+  const float d = P.depth[(size_t)y * P.depth_stride + (size_t)x * P.depth_comps];
+  if(!(d > 0.0f) || (__float_as_uint(d) & 0x7f800000u) == 0x7f800000u)   // not positive, or inf / NaN
+    return;
+  // depth is the distance along the ray, so the signed distance is taken along the ray too
+  const float r = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
+  const float sdf = __fsub_rn(d, r);
+  if(!(sdf >= -P.trunc))   // occluded (also drops NaN)
+    return;
+  const float o = fminf(1.0f, __fdiv_rn(sdf, P.trunc));
+  const size_t lin = ((size_t)k * g.ny + j) * g.nx + i;
+  const float2 rec = g.vox[lin];
+  const float w1 = __fadd_rn(rec.y, 1.0f);
+  const float t1 = __fdiv_rn(__fadd_rn(__fmul_rn(rec.x, rec.y), o), w1);
+  g.vox[lin] = make_float2(t1, fminf(w1, P.max_weight));
+}
+
+// ---------------------------------------------------------------------------------------- surface points
+__device__ __forceinline__ bool known_near_surface(float2 r)
+{
+  return r.y > 0.0f && fabsf(r.x) < 1.0f;
+}
+
+__device__ __forceinline__ bool crosses(float2 a, float2 b)
+{
+  return known_near_surface(b) && ((a.x > 0.0f && b.x <= 0.0f) || (a.x <= 0.0f && b.x > 0.0f));
+}
+
+// Voxel n and its +x, +y, +z neighbours: bit a of mask = a point on axis a.
+struct SurfaceCell
+{
+  float2 a, b[3];
+  int i, j, k;
+  unsigned int mask;
+};
+
+__device__ __forceinline__ SurfaceCell surface_cell(const VolumeGrid &g, unsigned int n, unsigned int n_vox)
+{
+  SurfaceCell c;
+  c.mask = 0u;
+  if(n >= n_vox)
+    return c;
+  c.a = __ldg(g.vox + n);
+  if(!known_near_surface(c.a))   // free space (tsdf 1) and unknown voxels: no neighbour loads
+    return c;
+  const unsigned int plane = (unsigned int)g.nx * (unsigned int)g.ny;
+  c.k = (int)(n / plane);
+  const unsigned int rem = n - (unsigned int)c.k * plane;
+  c.j = (int)(rem / (unsigned int)g.nx);
+  c.i = (int)(rem - (unsigned int)c.j * (unsigned int)g.nx);
+  if(c.i + 1 < g.nx)
+  {
+    c.b[0] = __ldg(g.vox + (size_t)n + 1);
+    c.mask |= crosses(c.a, c.b[0]) ? 1u : 0u;
+  }
+  if(c.j + 1 < g.ny)
+  {
+    c.b[1] = __ldg(g.vox + (size_t)n + g.nx);
+    c.mask |= crosses(c.a, c.b[1]) ? 2u : 0u;
+  }
+  if(c.k + 1 < g.nz)
+  {
+    c.b[2] = __ldg(g.vox + (size_t)n + plane);
+    c.mask |= crosses(c.a, c.b[2]) ? 4u : 0u;
+  }
+  return c;
+}
+
+// p_a + (t_a / (t_a - t_b)) * s along `axis`, weight min(w_a, w_b)
+__device__ __forceinline__ float4 surface_point(const VolumeGrid &g, const SurfaceCell &c, int axis)
+{
+  const float2 b = c.b[axis];
+  float4 o;
+  o.x = voxel_coord(g.ox, c.i, g.voxel);
+  o.y = voxel_coord(g.oy, c.j, g.voxel);
+  o.z = voxel_coord(g.oz, c.k, g.voxel);
+  const float step = __fmul_rn(__fdiv_rn(c.a.x, __fsub_rn(c.a.x, b.x)), g.voxel);
+  if(axis == 0) o.x = __fadd_rn(o.x, step);
+  else if(axis == 1) o.y = __fadd_rn(o.y, step);
+  else o.z = __fadd_rn(o.z, step);
+  o.w = fminf(c.a.y, b.y);
+  return o;
+}
+
+__device__ __forceinline__ unsigned int grid_voxels(const VolumeGrid &g)
+{
+  return (unsigned int)g.nx * (unsigned int)g.ny * (unsigned int)g.nz;   // <= 2^31
+}
+
+// Block b covers voxels [b * VOLUME_SURF_VOXELS, (b + 1) * VOLUME_SURF_VOXELS), in VOLUME_SURF_ROUNDS rounds of
+// VOLUME_SURF_BLOCK consecutive voxels (one per thread, so that loads coalesce).
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_count_kernel(const VolumeSurfaceParams P)
+{
+  __shared__ unsigned int warp_sum[VOLUME_SURF_BLOCK / 32];
+  const unsigned int n_vox = grid_voxels(P.g);
+  const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
+  unsigned int c = 0;
+#pragma unroll
+  for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
+    c += __popc(surface_cell(P.g, base + r * VOLUME_SURF_BLOCK, n_vox).mask);
+  c = __reduce_add_sync(0xffffffffu, c);
+  if((threadIdx.x & 31) == 0)
+    warp_sum[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if(threadIdx.x == 0)
+  {
+    unsigned int tot = 0;
+    for(int w = 0; w < VOLUME_SURF_BLOCK / 32; ++w) tot += warp_sum[w];
+    P.block_offsets[blockIdx.x] = tot;
+  }
+}
+
+// Second level: ONE block turns the block totals (up to 2^31 / VOLUME_SURF_VOXELS = 2^20 of them) into exclusive
+// offsets, VOLUME_SCAN_BLOCK * 8 totals per pass (8 consecutive per thread, then a block-wide scan of the sums).
+__global__ void __launch_bounds__(VOLUME_SCAN_BLOCK) volume_surface_scan_kernel(const VolumeSurfaceParams P)
+{
+  constexpr int PER = 8;
+  __shared__ unsigned long long warp_tot[VOLUME_SCAN_BLOCK / 32];
+  __shared__ unsigned long long carry;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if(threadIdx.x == 0)
+    carry = 0ull;
+  __syncthreads();
+  for(unsigned int b0 = 0; b0 < P.n_blocks; b0 += VOLUME_SCAN_BLOCK * PER)
+  {
+    const unsigned int first = b0 + threadIdx.x * PER;
+    unsigned long long v[PER], sum = 0ull;
+#pragma unroll
+    for(int q = 0; q < PER; ++q)
+    {
+      v[q] = (first + q < P.n_blocks) ? P.block_offsets[first + q] : 0ull;
+      sum += v[q];
+    }
+    unsigned long long inc = sum;
+#pragma unroll
+    for(int off = 1; off < 32; off <<= 1)
+    {
+      const unsigned long long up = __shfl_up_sync(0xffffffffu, inc, off);
+      if(lane >= off) inc += up;
+    }
+    if(lane == 31)
+      warp_tot[wid] = inc;
+    __syncthreads();
+    if(wid == 0)
+    {
+      unsigned long long w = warp_tot[lane];
+#pragma unroll
+      for(int off = 1; off < 32; off <<= 1)
+      {
+        const unsigned long long up = __shfl_up_sync(0xffffffffu, w, off);
+        if(lane >= off) w += up;
+      }
+      warp_tot[lane] = w;
+    }
+    __syncthreads();
+    unsigned long long run = carry + (wid ? warp_tot[wid - 1] : 0ull) + inc - sum;
+#pragma unroll
+    for(int q = 0; q < PER; ++q)
+    {
+      if(first + q < P.n_blocks)
+        P.block_offsets[first + q] = run;
+      run += v[q];
+    }
+    __syncthreads();   // every thread has read carry and warp_tot
+    if(threadIdx.x == VOLUME_SCAN_BLOCK - 1)
+      carry = run;     // the last thread's running sum ends at the pass total
+    __syncthreads();
+  }
+  if(threadIdx.x == 0)
+    P.total[0] = carry;
+}
+
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_write_kernel(const VolumeSurfaceParams P)
+{
+  __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const unsigned int n_vox = grid_voxels(P.g);
+  const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
+  unsigned long long rank = P.block_offsets[blockIdx.x];
+  for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
+  {
+    const SurfaceCell c = surface_cell(P.g, base + r * VOLUME_SURF_BLOCK, n_vox);
+    const unsigned int cnt = __popc(c.mask);
+    unsigned int inc = cnt;
+#pragma unroll
+    for(int off = 1; off < 32; off <<= 1)
+    {
+      const unsigned int up = __shfl_up_sync(0xffffffffu, inc, off);
+      if(lane >= off) inc += up;
+    }
+    if(lane == 31)
+      warp_off[wid] = inc;
+    __syncthreads();
+    unsigned int before = 0, all = 0;
+#pragma unroll
+    for(int w = 0; w < VOLUME_SURF_BLOCK / 32; ++w)
+    {
+      const unsigned int x = warp_off[w];
+      before += (w < wid) ? x : 0u;
+      all += x;
+    }
+    unsigned long long slot = rank + before + inc - cnt;
+#pragma unroll
+    for(int axis = 0; axis < 3; ++axis)
+    {
+      if(!(c.mask & (1u << axis)))
+        continue;
+      if(slot < P.capacity)
+        P.out[slot] = surface_point(P.g, c, axis);
+      ++slot;
+    }
+    rank += all;
+    __syncthreads();   // warp_off is reused by the next round
+  }
+}
+
+// --------------------------------------------------------------------------------------------- raycast
+__device__ __forceinline__ float lerp_rn(float a, float b, float f)
+{
+  return __fadd_rn(a, __fmul_rn(f, __fsub_rn(b, a)));
+}
+
+// Trilinear TSDF at grid coordinates (gx, gy, gz); false if a corner lies outside the grid or is unknown.
+__device__ __forceinline__ bool sample_tsdf(const VolumeGrid &g, float gx, float gy, float gz, float &out)
+{
+  const float x0 = floorf(gx), y0 = floorf(gy), z0 = floorf(gz);
+  const int i0 = (x0 >= 0.0f && x0 < 2.0e9f) ? (int)x0 : -1;
+  const int j0 = (y0 >= 0.0f && y0 < 2.0e9f) ? (int)y0 : -1;
+  const int k0 = (z0 >= 0.0f && z0 < 2.0e9f) ? (int)z0 : -1;
+  if(i0 < 0 || j0 < 0 || k0 < 0 || i0 + 1 >= g.nx || j0 + 1 >= g.ny || k0 + 1 >= g.nz)
+    return false;
+  const size_t plane = (size_t)g.nx * g.ny;
+  const float2 *b = g.vox + ((size_t)k0 * g.ny + j0) * g.nx + i0;
+  const float2 c000 = __ldg(b), c100 = __ldg(b + 1), c010 = __ldg(b + g.nx), c110 = __ldg(b + g.nx + 1);
+  const float2 c001 = __ldg(b + plane), c101 = __ldg(b + plane + 1), c011 = __ldg(b + plane + g.nx),
+               c111 = __ldg(b + plane + g.nx + 1);
+  if(c000.y == 0.0f || c100.y == 0.0f || c010.y == 0.0f || c110.y == 0.0f || c001.y == 0.0f || c101.y == 0.0f ||
+     c011.y == 0.0f || c111.y == 0.0f)
+    return false;
+  const float fx = __fsub_rn(gx, x0), fy = __fsub_rn(gy, y0), fz = __fsub_rn(gz, z0);
+  const float c00 = lerp_rn(c000.x, c100.x, fx), c10 = lerp_rn(c010.x, c110.x, fx);
+  const float c01 = lerp_rn(c001.x, c101.x, fx), c11 = lerp_rn(c011.x, c111.x, fx);
+  out = lerp_rn(lerp_rn(c00, c10, fy), lerp_rn(c01, c11, fy), fz);
+  return true;
+}
+
+__global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycastParams P)
+{
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const int y = blockIdx.y * blockDim.y + threadIdx.y;
+  if(x >= P.width || y >= P.height)
+    return;
+  const VolumeGrid &g = P.g;
+  // the ray of back_project (point_cloud.cuh), rotated into the world; it starts at the camera centre
+  const float vx = __fdiv_rn(__fsub_rn((float)x, P.cam.cx), P.cam.fx);
+  const float vy = __fdiv_rn(__fsub_rn((float)y, P.cam.cy), P.cam.fy);
+  const float dot = __fadd_rn(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)), 1.0f);
+  const float inv_len = __fdiv_rn(1.0f, __fsqrt_rn(dot));
+  const float qx = __fmul_rn(vx, inv_len), qy = __fmul_rn(vy, inv_len), qz = __fmul_rn(1.0f, inv_len);
+  const float *T = P.T_world_curr.m;
+  const float dir[3] = {__fadd_rn(__fadd_rn(__fmul_rn(T[0], qx), __fmul_rn(T[1], qy)), __fmul_rn(T[2], qz)),
+                        __fadd_rn(__fadd_rn(__fmul_rn(T[4], qx), __fmul_rn(T[5], qy)), __fmul_rn(T[6], qz)),
+                        __fadd_rn(__fadd_rn(__fmul_rn(T[8], qx), __fmul_rn(T[9], qy)), __fmul_rn(T[10], qz))};
+  const float org[3] = {T[3], T[7], T[11]};
+  const float lo[3] = {g.ox, g.oy, g.oz};
+  const int n[3] = {g.nx, g.ny, g.nz};
+  // slab test against the box of the voxel centres
+  float t0 = 0.0f, t1 = __int_as_float(0x7f800000);
+  bool inside = true;
+#pragma unroll
+  for(int a = 0; a < 3; ++a)
+  {
+    const float hi = voxel_coord(lo[a], n[a] - 1, g.voxel);
+    if(dir[a] == 0.0f)
+    {
+      inside = inside && org[a] >= lo[a] && org[a] <= hi;
+      continue;
+    }
+    const float ta = __fdiv_rn(__fsub_rn(lo[a], org[a]), dir[a]);
+    const float tb = __fdiv_rn(__fsub_rn(hi, org[a]), dir[a]);
+    t0 = fmaxf(t0, fminf(ta, tb));
+    t1 = fminf(t1, fmaxf(ta, tb));
+  }
+  float out = 0.0f;
+  if(inside && t0 <= t1)
+  {
+    // a segment inside the box is at most nx + ny + nz voxels long: the bound only stops a ray whose steps
+    // vanish against t0 (a camera very far away)
+    const int k_max = g.nx + g.ny + g.nz;
+    const float s = g.voxel;
+    bool prev_known = false;
+    float t_prev = 0.0f, f_prev = 0.0f;
+    for(int k = 0; k <= k_max; ++k)
+    {
+      const float t = __fadd_rn(t0, __fmul_rn((float)k, s));   // never accumulated
+      if(!(t <= t1))
+        break;
+      const float gx = __fdiv_rn(__fsub_rn(__fadd_rn(org[0], __fmul_rn(t, dir[0])), g.ox), s);
+      const float gy = __fdiv_rn(__fsub_rn(__fadd_rn(org[1], __fmul_rn(t, dir[1])), g.oy), s);
+      const float gz = __fdiv_rn(__fsub_rn(__fadd_rn(org[2], __fmul_rn(t, dir[2])), g.oz), s);
+      float f = 0.0f;
+      const bool known = sample_tsdf(g, gx, gy, gz, f);
+      if(known && prev_known && f_prev > 0.0f && f <= 0.0f)
+      {
+        out = __fadd_rn(t_prev, __fdiv_rn(__fmul_rn(s, f_prev), __fsub_rn(f_prev, f)));
+        break;
+      }
+      prev_known = known;
+      t_prev = t;
+      f_prev = f;
+    }
+  }
+  P.depth[(size_t)y * P.depth_stride + x] = out;
+}
+
+} // namespace
+
+cudaError_t launch_volume_integrate(const VolumeIntegrateParams &P, cudaStream_t stream)
+{
+  const unsigned int n = (unsigned int)P.g.nx * (unsigned int)P.g.ny * (unsigned int)P.g.nz;
+  volume_integrate_kernel<<<(n + 255u) / 256u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_surface_count(const VolumeSurfaceParams &P, cudaStream_t stream)
+{
+  volume_surface_count_kernel<<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  cudaError_t err = cudaGetLastError();
+  if(err != cudaSuccess) return err;
+  volume_surface_scan_kernel<<<1, VOLUME_SCAN_BLOCK, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_surface_write(const VolumeSurfaceParams &P, cudaStream_t stream)
+{
+  volume_surface_write_kernel<<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_raycast(const VolumeRaycastParams &P, cudaStream_t stream)
+{
+  const dim3 block(32, 8);
+  const dim3 grid((P.width + block.x - 1) / block.x, (P.height + block.y - 1) / block.y);
+  volume_raycast_kernel<<<grid, block, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+} // namespace rmdb

@@ -17,7 +17,7 @@ from typing import Callable, List, Optional
 
 import numpy as np
 
-from .api import PRIOR_SIGMA_SQ_FRAC, SE3, Depthmap, SeedMatrix
+from .api import PRIOR_SIGMA_SQ_FRAC, SE3, Depthmap, SeedMatrix, TsdfVolume
 
 UPDATE, TAKE_REFERENCE_FRAME = 0, 1   # rmd::ProcessingStates::State, include/rmd/depthmap_node.h:32-36
 
@@ -29,8 +29,10 @@ class DepthmapNode:
     (:157-161, :175-183)."""
 
     def __init__(self, depthmap: Depthmap, ref_compl_perc: float = 10.0, max_dist_from_ref: float = 0.5,
-                 publish_conv_every_n: int = 10, publisher: Optional[Callable] = None):
+                 publish_conv_every_n: int = 10, publisher: Optional[Callable] = None,
+                 volume: Optional[TsdfVolume] = None):
         self.depthmap_ = depthmap
+        self.volume_ = volume   # when given, every finished keyframe is fused into it (DESIGN.md 4.8)
         self.state_ = TAKE_REFERENCE_FRAME                      # src/depthmap_node.cpp:35
         self.ref_compl_perc_ = float(ref_compl_perc)            # :81, default 10.0
         self.max_dist_from_ref_ = float(max_dist_from_ref)      # :82, default 0.5
@@ -58,7 +60,11 @@ class DepthmapNode:
             self.num_msgs_ = 0
 
     def denoiseAndPublishResults(self) -> None:
-        self.depthmap_.downloadDenoisedDepthmap(0.5, 200)                         # :167
+        if self.volume_ is not None:
+            # the same host map as downloadDenoisedDepthmap, and the keyframe fused from the device copy
+            self.depthmap_.fuseDenoisedInto(self.volume_, 0.5, 200)
+        else:
+            self.depthmap_.downloadDenoisedDepthmap(0.5, 200)                     # :167
         self.depthmap_.downloadConvergenceMap()                                   # :168
         if self.publisher_:
             self.publisher_("depthmap_and_pointcloud", self.depthmap_)
