@@ -5,6 +5,7 @@
 #define TSDF_VOLUME_CUH
 
 #include <cstddef>
+#include <cstdint>
 #include <vector>
 
 #include <rmd/pinhole_camera.cuh>
@@ -57,6 +58,21 @@ public:
                              "TsdfVolume: unable to extract points");
     out.resize(4 * n < out.size() ? 4 * n : out.size());
     return out;
+  }
+
+  // Triangle mesh of the fused surface: xyzw = surfacePoints() (4 floats per vertex), tri = 3 vertex indices per
+  // triangle, (b - a) x (c - a) towards free space.  Throws for 2^31 or more vertices.
+  void mesh(std::vector<float> &xyzw, std::vector<int32_t> &tri)
+  {
+    size_t nv = 0, nt = 0;
+    detail::throw_on_error(rmd_volume_mesh(handle_, NULL, 0, NULL, 0, &nv, &nt), "TsdfVolume: unable to count the mesh");
+    xyzw.resize(4 * nv);
+    tri.resize(3 * nt);
+    if(nv || nt)
+      detail::throw_on_error(rmd_volume_mesh(handle_, xyzw.data(), nv, tri.data(), nt, &nv, &nt),
+                             "TsdfVolume: unable to extract the mesh");
+    xyzw.resize(4 * nv < xyzw.size() ? 4 * nv : xyzw.size());
+    tri.resize(3 * nt < tri.size() ? 3 * nt : tri.size());
   }
 
   // Distance along each pixel's ray to the fused surface (0 = none) into a pitched device image; asynchronous on

@@ -464,6 +464,35 @@ int rmd_volume_surface_points(rmd_volume_t *v, float *host_xyzw, size_t capacity
 /* Same into device memory (16-byte aligned). */
 int rmd_volume_surface_points_device(rmd_volume_t *v, float *dev_xyzw, size_t capacity, size_t *count);
 
+/* The surface as an indexed, watertight triangle mesh (marching cubes with a
+ * generated case table, DESIGN.md 4.8).  The vertices ARE the surface points:
+ * the same array, bit for bit, as rmd_volume_surface_points.  Cube (i, j, k),
+ * i < nx-1, j < ny-1, k < nz-1, has corner c = dx + 2 dy + 4 dz at voxel
+ * (i+dx, j+dy, k+dz); a corner is inside when tsdf <= 0.  A cube is meshed
+ * only when its 8 corners have weight > 0 and every cube edge whose ends differ
+ * in sign has |tsdf| < 1 at both ends; its triangles then use exactly the
+ * surface points on its crossing edges.  Triangles are 3 int32 vertex indices,
+ * ordered by cube index, then by the table; (b - a) x (c - a) points to the
+ * tsdf > 0 side (free space, the cameras).  Two cubes sharing a face cut it
+ * the same way (on a face with four crossings each inside corner is cut off),
+ * so the mesh is closed except at unknown / truncated cubes and the grid's
+ * outer faces.
+ *
+ * *n_vertices and *n_triangles are always written; at most vertex_capacity
+ * vertices (4 floats x, y, z, w each) and tri_capacity triangles are written.
+ * Triangles may reference vertices beyond vertex_capacity.  NULL buffers with
+ * capacity 0 only count.  The host variant stages what it writes in device
+ * memory it keeps (grown on demand); the mesh path also keeps 8 B of scratch
+ * per vertex.  Synchronous.  RMD_ERR_INVALID_ARGUMENT: null handle or count
+ * pointer, null buffer with capacity > 0; for the device variant also a vertex
+ * buffer not 16-byte aligned or a triangle buffer not 4-byte aligned.
+ * RMD_ERR_UNSUPPORTED: 2^31 or more vertices (int32 indices); both counts are
+ * still written and nothing else is. */
+int rmd_volume_mesh(rmd_volume_t *v, float *host_xyzw, size_t vertex_capacity, int32_t *host_tri,
+                    size_t tri_capacity, size_t *n_vertices, size_t *n_triangles);
+int rmd_volume_mesh_device(rmd_volume_t *v, float *dev_xyzw, size_t vertex_capacity, int32_t *dev_tri,
+                           size_t tri_capacity, size_t *n_vertices, size_t *n_triangles);
+
 /* Depth map of the fused surface seen by the pinhole camera (fx, fy, cx, cy)
  * at T_curr_world: the ray of pixel (x, y), normalize((x-cx)/fx, (y-cy)/fy,
  * 1) rotated into the world from the camera centre, is clipped to the box of

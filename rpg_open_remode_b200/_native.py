@@ -81,6 +81,8 @@ _SIGNATURES = {
     "rmd_volume_integrate_depth": (ci, [vp, ci, ci, cf, cf, cf, cf, vp, vp, cs, vp, cs]),
     "rmd_volume_surface_points": (ci, [vp, vp, cs, P(cs)]),
     "rmd_volume_surface_points_device": (ci, [vp, vp, cs, P(cs)]),
+    "rmd_volume_mesh": (ci, [vp, vp, cs, vp, cs, P(cs), P(cs)]),
+    "rmd_volume_mesh_device": (ci, [vp, vp, cs, vp, cs, P(cs), P(cs)]),
     "rmd_volume_raycast": (ci, [vp, ci, ci, cf, cf, cf, cf, vp, vp, cs]),
     "rmd_volume_download": (ci, [vp, vp, vp]),
     "rmd_volume_upload": (ci, [vp, vp, vp]),

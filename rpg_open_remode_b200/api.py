@@ -571,6 +571,24 @@ class TsdfVolume:
                                                 ctypes.byref(n)), "TsdfVolume::surfacePoints")
         return out[:min(int(capacity), n.value)]
 
+    def mesh(self, vertex_capacity: "int | None" = None, triangle_capacity: "int | None" = None):
+        """Marching-cubes mesh of the fused surface: (float32 [n, 4] vertices, int32 [m, 3] triangles).  The vertices
+        are surfacePoints(), bit for bit; triangles are ordered by cube and face the tsdf > 0 side, (b - a) x (c - a).
+        With capacities, at most that many of each (triangles may then index vertices that were not returned).
+        Raises RmdError (RMD_ERR_UNSUPPORTED) for 2^31 or more vertices."""
+        nv, nt = ctypes.c_size_t(), ctypes.c_size_t()
+        if vertex_capacity is None or triangle_capacity is None:
+            check(self._L.rmd_volume_mesh(self._h, None, 0, None, 0, ctypes.byref(nv), ctypes.byref(nt)),
+                  "TsdfVolume::mesh")
+            vertex_capacity = nv.value if vertex_capacity is None else vertex_capacity
+            triangle_capacity = nt.value if triangle_capacity is None else triangle_capacity
+        verts = np.empty((int(vertex_capacity), 4), np.float32)
+        tris = np.empty((int(triangle_capacity), 3), np.int32)
+        check(self._L.rmd_volume_mesh(self._h, verts.ctypes.data if vertex_capacity else None, int(vertex_capacity),
+                                      tris.ctypes.data if triangle_capacity else None, int(triangle_capacity),
+                                      ctypes.byref(nv), ctypes.byref(nt)), "TsdfVolume::mesh")
+        return verts[:min(int(vertex_capacity), nv.value)], tris[:min(int(triangle_capacity), nt.value)]
+
     def raycast(self, cam: PinholeCamera, T_curr_world, width: int, height: int) -> np.ndarray:
         """float32 [height, width]: distance along each pixel's ray to the fused surface, 0 where none."""
         img = DeviceImage(width, height, "float32")
@@ -602,6 +620,22 @@ class TsdfVolume:
 
     def sync(self) -> None:
         check(self._L.rmd_volume_sync(self._h), "TsdfVolume::sync")
+
+
+def write_ply(path: str, vertices, triangles) -> None:
+    """Binary little-endian PLY of a mesh such as TsdfVolume.mesh() returns: per vertex float x, y, z and the
+    weight as float `weight`; per face a uchar-counted int list `vertex_indices`."""
+    v = np.ascontiguousarray(vertices, "<f4").reshape(-1, 4)
+    t = np.ascontiguousarray(triangles, "<i4").reshape(-1, 3)
+    faces = np.empty(len(t), np.dtype([("n", "u1"), ("i", "<i4", 3)]))
+    faces["n"], faces["i"] = 3, t
+    header = ("ply\nformat binary_little_endian 1.0\n"
+              "element vertex %d\nproperty float x\nproperty float y\nproperty float z\nproperty float weight\n"
+              "element face %d\nproperty list uchar int vertex_indices\nend_header\n" % (len(v), len(t)))
+    with open(path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(v.tobytes())
+        f.write(faces.tobytes())
 
 
 class ImageReducer:

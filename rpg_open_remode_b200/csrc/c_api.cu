@@ -2090,6 +2090,11 @@ struct rmd_volume
   // surface points (allocated on first use): per-block offsets, total, host staging grown on demand
   unsigned long long *surf_offsets, *surf_total;
   float4 *stage; size_t stage_cap;
+  // mesh (allocated on first use): per-block triangle offsets and total, the points' keys and the host variant's
+  // triangle staging, grown on demand
+  unsigned long long *tri_offsets, *tri_total;
+  unsigned long long *keys; size_t keys_cap;
+  int *tri_stage; size_t tri_stage_cap;
   uint64_t n_total;
 };
 
@@ -2152,6 +2157,105 @@ int volume_surface_write(rmd_volume *v, VolumeSurfaceParams &P, float4 *out, siz
   return 0;
 }
 
+// Device buffer of at least n elements, grown (never shrunk) on demand.
+template<typename T>
+int volume_grow(T **buf, size_t *cap, size_t n)
+{
+  if(n <= *cap)
+    return 0;
+  RMD_CUDA_TRY(cudaFree(*buf));
+  *buf = NULL; *cap = 0;
+  RMD_CUDA_TRY(cudaMalloc(buf, sizeof(T) * n));
+  *cap = n;
+  return 0;
+}
+
+// The mesh: both count passes and scans, one host read of the two totals, then -- for what the capacities ask --
+// the surface points (with their keys when triangles are wanted) and the triangles.  host: min(count, capacity)
+// of each are staged in the volume's buffers and copied to xyzw / tri.  Synchronous.
+int volume_mesh(rmd_volume *v, void *xyzw, size_t vertex_capacity, int32_t *tri, size_t tri_capacity,
+                size_t *n_vertices, size_t *n_triangles, bool host, const char *what)
+{
+  VolumeSurfaceParams S;
+  memset(&S, 0, sizeof(S));
+  S.g = v->g;
+  S.n_blocks = (unsigned int)((v->n_vox + VOLUME_SURF_VOXELS - 1) / VOLUME_SURF_VOXELS);
+  if(!v->surf_offsets)
+  {
+    RMD_CUDA_TRY(cudaMalloc(&v->surf_offsets, sizeof(unsigned long long) * S.n_blocks));
+    RMD_CUDA_TRY(cudaMalloc(&v->surf_total, sizeof(unsigned long long)));
+  }
+  if(!v->tri_offsets)
+  {
+    RMD_CUDA_TRY(cudaMalloc(&v->tri_offsets, sizeof(unsigned long long) * S.n_blocks));
+    RMD_CUDA_TRY(cudaMalloc(&v->tri_total, sizeof(unsigned long long)));
+  }
+  S.block_offsets = v->surf_offsets;
+  S.total = v->surf_total;
+  VolumeMeshParams M;
+  memset(&M, 0, sizeof(M));
+  M.g = v->g;
+  M.point_offsets = v->surf_offsets;
+  M.point_total = v->surf_total;
+  M.block_offsets = v->tri_offsets;
+  M.total = v->tri_total;
+  M.n_blocks = S.n_blocks;
+  RMD_CUDA_TRY(launch_volume_surface_count(S, v->stream));
+  RMD_CUDA_TRY(launch_volume_mesh_count(M, v->stream));
+  v->n_total += 4;
+  unsigned long long nv = 0, nt = 0;
+  RMD_CUDA_TRY(cudaMemcpyAsync(&nv, v->surf_total, sizeof(nv), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaMemcpyAsync(&nt, v->tri_total, sizeof(nt), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  *n_vertices = (size_t)nv;
+  *n_triangles = (size_t)nt;
+  if(nv >= (1ull << 31))
+    return fail(RMD_ERR_UNSUPPORTED, (std::string(what) + ": 2^31 or more vertices do not fit int32 indices").c_str());
+  const size_t mv = nv < vertex_capacity ? (size_t)nv : vertex_capacity;
+  const size_t mt = nt < tri_capacity ? (size_t)nt : tri_capacity;
+  if(!mv && !mt)
+    return 0;
+  float4 *vout = reinterpret_cast<float4*>(xyzw);
+  int *tout = tri;
+  if(host)
+  {
+    int rc = volume_grow(&v->stage, &v->stage_cap, mv);
+    if(!rc) rc = volume_grow(&v->tri_stage, &v->tri_stage_cap, 3 * mt);
+    if(rc) return rc;
+    vout = v->stage;
+    tout = v->tri_stage;
+  }
+  S.out = vout;
+  S.capacity = mv;
+  if(mt)
+  {
+    // every vertex's key, whatever the vertex capacity: triangles may index vertices that are not returned
+    const int rc = volume_grow(&v->keys, &v->keys_cap, (size_t)nv);
+    if(rc) return rc;
+    S.keys = v->keys;
+    RMD_CUDA_TRY(launch_volume_surface_write_keys(S, v->stream));
+    M.keys = v->keys;
+    M.tri = tout;
+    M.capacity = mt;
+    RMD_CUDA_TRY(launch_volume_mesh_write(M, v->stream));
+    v->n_total += 2;
+  }
+  else
+  {
+    RMD_CUDA_TRY(launch_volume_surface_write(S, v->stream));
+    v->n_total += 1;
+  }
+  if(host)
+  {
+    if(mv)
+      RMD_CUDA_TRY(cudaMemcpyAsync(xyzw, v->stage, mv * sizeof(float4), cudaMemcpyDeviceToHost, v->stream));
+    if(mt)
+      RMD_CUDA_TRY(cudaMemcpyAsync(tri, v->tri_stage, mt * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, v->stream));
+  }
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  return 0;
+}
+
 } // namespace
 
 extern "C"
@@ -2206,6 +2310,7 @@ int rmd_volume_destroy(rmd_volume_t *v)
   if(v->seeds_ev) cudaEventDestroy(v->seeds_ev);
   cudaFree(v->g.vox);
   cudaFree(v->surf_offsets); cudaFree(v->surf_total); cudaFree(v->stage);
+  cudaFree(v->tri_offsets); cudaFree(v->tri_total); cudaFree(v->keys); cudaFree(v->tri_stage);
   cudaGetLastError();
   delete v;
   return 0;
@@ -2336,6 +2441,28 @@ int rmd_volume_surface_points_device(rmd_volume_t *v, float *dev_xyzw, size_t ca
   }
   RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
   return 0;
+}
+
+int rmd_volume_mesh(rmd_volume_t *v, float *host_xyzw, size_t vertex_capacity, int32_t *host_tri,
+                    size_t tri_capacity, size_t *n_vertices, size_t *n_triangles)
+{
+  RMD_REQUIRE(v && n_vertices && n_triangles && (host_xyzw || vertex_capacity == 0) && (host_tri || tri_capacity == 0),
+              "rmd_volume_mesh: null argument");
+  DeviceGuard guard(v->device);
+  return volume_mesh(v, host_xyzw, vertex_capacity, host_tri, tri_capacity, n_vertices, n_triangles, true,
+                     "rmd_volume_mesh");
+}
+
+int rmd_volume_mesh_device(rmd_volume_t *v, float *dev_xyzw, size_t vertex_capacity, int32_t *dev_tri,
+                           size_t tri_capacity, size_t *n_vertices, size_t *n_triangles)
+{
+  RMD_REQUIRE(v && n_vertices && n_triangles && (dev_xyzw || vertex_capacity == 0) && (dev_tri || tri_capacity == 0),
+              "rmd_volume_mesh_device: null argument");
+  RMD_REQUIRE(((uintptr_t)dev_xyzw % 16) == 0, "rmd_volume_mesh_device: vertices must be 16-byte aligned");
+  RMD_REQUIRE(((uintptr_t)dev_tri % 4) == 0, "rmd_volume_mesh_device: triangles must be 4-byte aligned");
+  DeviceGuard guard(v->device);
+  return volume_mesh(v, dev_xyzw, vertex_capacity, dev_tri, tri_capacity, n_vertices, n_triangles, false,
+                     "rmd_volume_mesh_device");
 }
 
 int rmd_volume_raycast(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,

@@ -2,6 +2,11 @@
 // raycast reads the few voxels around each ray through the read-only path.
 #include "volume.cuh"
 
+#include <cstring>
+
+#define RMD_MC_STORAGE static __constant__
+#include "mc_table.h"
+
 namespace rmdb
 {
 
@@ -213,6 +218,8 @@ __global__ void __launch_bounds__(VOLUME_SCAN_BLOCK) volume_surface_scan_kernel(
     P.total[0] = carry;
 }
 
+// KEYS (the mesh path): also write every point's key 3 * voxel + axis, for all *total points whatever the capacity.
+template<bool KEYS>
 __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_write_kernel(const VolumeSurfaceParams P)
 {
   __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
@@ -250,7 +257,135 @@ __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_write_kernel
         continue;
       if(slot < P.capacity)
         P.out[slot] = surface_point(P.g, c, axis);
+      if(KEYS)
+        P.keys[slot] = 3ull * (base + r * VOLUME_SURF_BLOCK) + axis;
       ++slot;
+    }
+    rank += all;
+    __syncthreads();   // warp_off is reused by the next round
+  }
+}
+
+// --------------------------------------------------------------------------------------------------- mesh
+// Case of cube n (corner c = dx + 2 dy + 4 dz at voxel n + dx + dy nx + dz nx ny; bit c = inside, tsdf <= 0), or 0
+// when the cube is not meshed.  An unknown lower corner costs one load; the other seven corners come from the same
+// row (L1) and the +y / +z rows and planes, which the neighbouring blocks stream through L2.
+__device__ __forceinline__ unsigned int mesh_cube(const VolumeGrid &g, unsigned int n, unsigned int n_vox)
+{
+  if(n >= n_vox)
+    return 0u;
+  const float2 a = __ldg(g.vox + n);
+  if(!(a.y > 0.0f))
+    return 0u;
+  const unsigned int plane = (unsigned int)g.nx * (unsigned int)g.ny;
+  const unsigned int k = n / plane;
+  const unsigned int rem = n - k * plane;
+  const unsigned int j = rem / (unsigned int)g.nx;
+  const unsigned int i = rem - j * (unsigned int)g.nx;
+  if(i + 1u >= (unsigned int)g.nx || j + 1u >= (unsigned int)g.ny || k + 1u >= (unsigned int)g.nz)
+    return 0u;
+  const float2 *p = g.vox + n;
+  const size_t sy = (size_t)g.nx, sz = (size_t)plane;
+  const float2 r[8] = {a, __ldg(p + 1), __ldg(p + sy), __ldg(p + sy + 1), __ldg(p + sz), __ldg(p + sz + 1),
+                       __ldg(p + sz + sy), __ldg(p + sz + sy + 1)};
+  unsigned int cube = 0u, near = 0u;
+  bool known = true;
+#pragma unroll
+  for(int c = 0; c < 8; ++c)
+  {
+    known = known && r[c].y > 0.0f;
+    cube |= (r[c].x <= 0.0f ? 1u : 0u) << c;
+    near |= (fabsf(r[c].x) < 1.0f ? 1u : 0u) << c;
+  }
+  if(!known || cube == 0u || cube == 255u)
+    return 0u;
+  // a crossing edge (ends differ in sign) with a truncated end: x edges pair corners c, c + 1 (mask 0x55), y edges
+  // c, c + 2 (0x33), z edges c, c + 4 (0x0f)
+  const unsigned int bad = (((cube ^ (cube >> 1)) & ~(near & (near >> 1))) & 0x55u) |
+                           (((cube ^ (cube >> 2)) & ~(near & (near >> 2))) & 0x33u) |
+                           (((cube ^ (cube >> 4)) & ~(near & (near >> 4))) & 0x0fu);
+  return bad ? 0u : cube;
+}
+
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_mesh_count_kernel(const VolumeMeshParams P)
+{
+  __shared__ unsigned int warp_sum[VOLUME_SURF_BLOCK / 32];
+  const unsigned int n_vox = grid_voxels(P.g);
+  const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
+  unsigned int c = 0;
+#pragma unroll
+  for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
+    c += RMD_MC_NTRI[mesh_cube(P.g, base + r * VOLUME_SURF_BLOCK, n_vox)];
+  c = __reduce_add_sync(0xffffffffu, c);
+  if((threadIdx.x & 31) == 0)
+    warp_sum[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if(threadIdx.x == 0)
+  {
+    unsigned int tot = 0;
+    for(int w = 0; w < VOLUME_SURF_BLOCK / 32; ++w) tot += warp_sum[w];
+    P.block_offsets[blockIdx.x] = tot;
+  }
+}
+
+// Index of the surface point on edge e of cube n: binary search for its key among the points of the edge's voxel's
+// block, [offset[b], offset[b + 1]) -- at most 3 * VOLUME_SURF_VOXELS = 6144 keys, 13 steps.  The point exists: the
+// cube test is the surface-point rule on every crossing edge.
+__device__ __forceinline__ int mesh_vertex(const VolumeMeshParams &P, unsigned int n, int e)
+{
+  const unsigned int c0 = RMD_MC_EDGE[e][0], axis = RMD_MC_EDGE[e][1];
+  const unsigned int v = n + (c0 & 1u) + ((c0 >> 1) & 1u) * (unsigned int)P.g.nx +
+                         ((c0 >> 2) & 1u) * (unsigned int)P.g.nx * (unsigned int)P.g.ny;   // a voxel: < 2^31
+  const unsigned long long key = 3ull * v + axis;
+  const unsigned int b = v / VOLUME_SURF_VOXELS;
+  unsigned long long lo = P.point_offsets[b];
+  unsigned long long hi = b + 1 < P.n_blocks ? P.point_offsets[b + 1] : P.point_total[0];
+  while(lo < hi)
+  {
+    const unsigned long long mid = (lo + hi) >> 1;
+    if(P.keys[mid] < key) lo = mid + 1;
+    else hi = mid;
+  }
+  return (int)lo;   // < 2^31 points (the host refuses more)
+}
+
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_mesh_write_kernel(const VolumeMeshParams P)
+{
+  __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const unsigned int n_vox = grid_voxels(P.g);
+  const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
+  unsigned long long rank = P.block_offsets[blockIdx.x];
+  for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
+  {
+    const unsigned int n = base + r * VOLUME_SURF_BLOCK;
+    const unsigned int cube = mesh_cube(P.g, n, n_vox);
+    const unsigned int cnt = RMD_MC_NTRI[cube];
+    unsigned int inc = cnt;
+#pragma unroll
+    for(int off = 1; off < 32; off <<= 1)
+    {
+      const unsigned int up = __shfl_up_sync(0xffffffffu, inc, off);
+      if(lane >= off) inc += up;
+    }
+    if(lane == 31)
+      warp_off[wid] = inc;
+    __syncthreads();
+    unsigned int before = 0, all = 0;
+#pragma unroll
+    for(int w = 0; w < VOLUME_SURF_BLOCK / 32; ++w)
+    {
+      const unsigned int x = warp_off[w];
+      before += (w < wid) ? x : 0u;
+      all += x;
+    }
+    unsigned long long slot = rank + before + inc - cnt;
+    for(unsigned int q = 0; q < cnt && slot < P.capacity; ++q, ++slot)
+    {
+      int *t = P.tri + 3 * slot;
+      t[0] = mesh_vertex(P, n, RMD_MC_TRIS[cube][3 * q + 0]);
+      t[1] = mesh_vertex(P, n, RMD_MC_TRIS[cube][3 * q + 1]);
+      t[2] = mesh_vertex(P, n, RMD_MC_TRIS[cube][3 * q + 2]);
     }
     rank += all;
     __syncthreads();   // warp_off is reused by the next round
@@ -376,7 +511,34 @@ cudaError_t launch_volume_surface_count(const VolumeSurfaceParams &P, cudaStream
 
 cudaError_t launch_volume_surface_write(const VolumeSurfaceParams &P, cudaStream_t stream)
 {
-  volume_surface_write_kernel<<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  volume_surface_write_kernel<false><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_surface_write_keys(const VolumeSurfaceParams &P, cudaStream_t stream)
+{
+  volume_surface_write_kernel<true><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_mesh_count(const VolumeMeshParams &P, cudaStream_t stream)
+{
+  volume_mesh_count_kernel<<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  cudaError_t err = cudaGetLastError();
+  if(err != cudaSuccess) return err;
+  VolumeSurfaceParams S;   // the surface points' block-total scan, on the triangle totals
+  memset(&S, 0, sizeof(S));
+  S.g = P.g;
+  S.block_offsets = P.block_offsets;
+  S.total = P.total;
+  S.n_blocks = P.n_blocks;
+  volume_surface_scan_kernel<<<1, VOLUME_SCAN_BLOCK, 0, stream>>>(S);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_mesh_write(const VolumeMeshParams &P, cudaStream_t stream)
+{
+  volume_mesh_write_kernel<<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   return cudaGetLastError();
 }
 

@@ -1,6 +1,6 @@
 """Device time of the TSDF volume's operations (DESIGN.md 4.8, 6) on bench.py's c2 scene (VGA): integration of one
-keyframe's depth and state map into a 256^3 and a 512^3 grid over the scene, surface-point extraction, and a VGA
-raycast.  Each time is the median of REPEATS runs after WARMUP, measured with CUDA events on the volume's stream.
+keyframe's depth and state map into a 256^3 and a 512^3 grid over the scene, surface-point extraction, the
+triangle mesh (rmd_volume_mesh_device, vertices and triangles) and a VGA raycast.  Each time is the median of REPEATS runs after WARMUP, measured with CUDA events on the volume's stream.
 The achieved bandwidth of an integration counts 16 B per updated voxel (record read + write) and 8 B per pixel
 (depth + state) over its kernel time, against the 3.35 TB/s of the H100 SXM data sheet.  Prints one JSON line with
 the GPU's name and power limit.  GPU box only."""
@@ -90,6 +90,15 @@ def main():
             _native.check(L.rmd_volume_surface_points_device(v.handle, points.data, 4 * n * n, ctypes.byref(count)))
 
         ms_pts, runs_pts = timed(stream, torch, extract)
+        n_tri = ctypes.c_size_t()
+        tris = rmd.DeviceImage(3 * 8 * n * n, 1, "int32")         # room for 8 n^2 triangles
+
+        def mesh():
+            _native.check(L.rmd_volume_mesh_device(v.handle, points.data, 4 * n * n, tris.data, 8 * n * n,
+                                                   ctypes.byref(count), ctypes.byref(n_tri)))
+
+        ms_mesh, runs_mesh = timed(stream, torch, mesh)
+        assert count.value <= 4 * n * n and n_tri.value <= 8 * n * n
 
         def raycast():
             _native.check(L.rmd_volume_raycast(v.handle, W, H, c(cam.fx), c(cam.fy), c(cam.cx), c(cam.cy),
@@ -108,6 +117,8 @@ def main():
             "record_stream_bytes": 8 * n ** 3,
             "surface_points": int(count.value), "surface_points_ms": ms_pts, "surface_points_ms_runs": runs_pts,
             "surface_points_record_bandwidth_TBps": 8 * n ** 3 / (ms_pts * 1e-3) / 1e12,
+            "mesh_vertices": int(count.value), "mesh_triangles": int(n_tri.value), "mesh_ms": ms_mesh,
+            "mesh_ms_runs": runs_mesh, "mesh_over_surface_points": ms_mesh / ms_pts,
             "raycast_vga_ms": ms_ray, "raycast_vga_ms_runs": runs_ray, "raycast_pixels_hit": hit}
         del v
     try:
