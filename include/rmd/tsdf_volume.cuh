@@ -85,6 +85,58 @@ public:
                            "TsdfVolume: unable to raycast");
   }
 
+  // Intensity channel (8 B per voxel): from now on integrate() also fuses the keyframe's reference image.
+  void enableIntensity()
+  {
+    detail::throw_on_error(rmd_volume_enable_intensity(handle_), "TsdfVolume: unable to enable the intensity");
+  }
+
+  // integrateDepth plus a float intensity image of the same size, fused into the intensity channel.
+  void integrateDepthIntensity(int width, int height, const PinholeCamera &cam, const SE3<float> &T_curr_world,
+                               const float *dev_depth, size_t depth_pitch, const float *dev_intensity,
+                               size_t intensity_pitch, const int *dev_conv = NULL, size_t conv_pitch = 0)
+  {
+    detail::throw_on_error(rmd_volume_integrate_depth_intensity(handle_, width, height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                                                T_curr_world.data.data, dev_depth, depth_pitch,
+                                                                dev_conv, conv_pitch, dev_intensity,
+                                                                intensity_pitch),
+                           "TsdfVolume: unable to integrate the depth and intensity images");
+  }
+
+  // One intensity per surface point (= mesh vertex), in surfacePoints() order; -1 = none.
+  std::vector<float> surfaceIntensity()
+  {
+    size_t n = 0;
+    detail::throw_on_error(rmd_volume_surface_intensity(handle_, NULL, 0, &n), "TsdfVolume: unable to count points");
+    std::vector<float> out(n);
+    if(n)
+      detail::throw_on_error(rmd_volume_surface_intensity(handle_, out.data(), n, &n),
+                             "TsdfVolume: unable to extract the intensities");
+    out.resize(n < out.size() ? n : out.size());
+    return out;
+  }
+
+  // raycast() and the intensity at each hit (-1 = none) into two pitched device images; asynchronous.
+  void raycastIntensity(int width, int height, const PinholeCamera &cam, const SE3<float> &T_curr_world,
+                        float *dev_depth, size_t depth_pitch, float *dev_intensity, size_t intensity_pitch)
+  {
+    detail::throw_on_error(rmd_volume_raycast_intensity(handle_, width, height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                                        T_curr_world.data.data, dev_depth, depth_pitch,
+                                                        dev_intensity, intensity_pitch),
+                           "TsdfVolume: unable to raycast the intensity");
+  }
+
+  void downloadIntensity(float *host_intensity, float *host_weight)
+  {
+    detail::throw_on_error(rmd_volume_download_intensity(handle_, host_intensity, host_weight),
+                           "TsdfVolume: unable to download the intensity");
+  }
+  void uploadIntensity(const float *host_intensity, const float *host_weight)
+  {
+    detail::throw_on_error(rmd_volume_upload_intensity(handle_, host_intensity, host_weight),
+                           "TsdfVolume: unable to upload the intensity");
+  }
+
   void download(float *host_tsdf, float *host_weight)
   {
     detail::throw_on_error(rmd_volume_download(handle_, host_tsdf, host_weight), "TsdfVolume: unable to download");

@@ -510,6 +510,55 @@ int rmd_volume_raycast(rmd_volume_t *v, int width, int height, float fx, float f
 int rmd_volume_download(rmd_volume_t *v, float *host_tsdf, float *host_weight);
 int rmd_volume_upload(rmd_volume_t *v, const float *host_tsdf, const float *host_weight);
 
+/* Intensity channel (DESIGN.md 4.8): an opt-in second record per voxel,
+ * (intensity, weight), that fuses the images the depth maps were seen in, so
+ * that surface points, mesh vertices and raycast views can be shaded.  The
+ * (tsdf, weight) records, surface points, mesh and raycast depth of a volume
+ * are bit-identical with and without it.  Intensity is in the units of the
+ * images fused (for seeds: the reference image, 8-bit * 1/255); -1 = none.
+ *
+ * rmd_volume_enable_intensity allocates the channel (8 B per voxel) and
+ * zeroes it asynchronously on the volume's stream; a second call does
+ * nothing.  rmd_volume_reset also clears it.  Returns cudaErrorMemoryAllocation
+ * when it does not fit.  From then on rmd_volume_integrate_seeds also fuses
+ * s's reference image (ordered like the depth it reads); plain
+ * rmd_volume_integrate_depth leaves the channel untouched.
+ *
+ * Every intensity entry point below returns RMD_ERR_NOT_INITIALISED on a
+ * volume without the channel and RMD_ERR_INVALID_ARGUMENT for a null handle or
+ * pointer or a bad pitch (pitches in bytes, >= width * 4, a multiple of 4). */
+int rmd_volume_enable_intensity(rmd_volume_t *v);
+/* rmd_volume_integrate_depth, and then every updated voxel in the band
+ * (sdf < tau, so -tau <= sdf < tau) whose pixel (x, y) -- the depth's -- has a
+ * finite intensity I in dev_intensity (float, the depth's size) gets
+ * wc' = wc + 1,  c' = (c wc + I) / wc',  stored as (c', min(wc', max_weight)).
+ * Free space (o = 1) does not take the colour of what lies behind it.
+ * Asynchronous on the volume's stream. */
+int rmd_volume_integrate_depth_intensity(rmd_volume_t *v, int width, int height, float fx, float fy, float cx,
+                                         float cy, const float *T_curr_world, const float *dev_depth,
+                                         size_t depth_pitch, const int32_t *dev_conv, size_t conv_pitch,
+                                         const float *dev_intensity, size_t intensity_pitch);
+/* One float per surface point, in rmd_volume_surface_points' order and count
+ * (and so per mesh vertex): with f = t_a / (t_a - t_b), the point's factor,
+ * c_a + f (c_b - c_a) when both voxels' intensity weights are > 0, the
+ * intensity of the one that is > 0, else -1.  Same count / capacity / staging
+ * contract as rmd_volume_surface_points[_device] (device output 4-byte
+ * aligned).  Synchronous. */
+int rmd_volume_surface_intensity(rmd_volume_t *v, float *host_intensity, size_t capacity, size_t *count);
+int rmd_volume_surface_intensity_device(rmd_volume_t *v, float *dev_intensity, size_t capacity, size_t *count);
+/* rmd_volume_raycast (dev_depth bit-identical to it) and, per pixel, the
+ * intensity at the hit t: grid coordinates of org + t dir as the march
+ * computes them, trilinear interpolation in x, then y, then z of the 8
+ * intensity records around it; -1 when one of them lies outside the grid or
+ * has weight 0, and where there is no hit (depth 0).  Asynchronous on the
+ * volume's stream. */
+int rmd_volume_raycast_intensity(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                                 const float *T_curr_world, float *dev_depth, size_t depth_pitch,
+                                 float *dev_intensity, size_t intensity_pitch);
+/* Test / checkpoint hooks of the channel, like rmd_volume_download / upload. */
+int rmd_volume_download_intensity(rmd_volume_t *v, float *host_intensity, float *host_weight);
+int rmd_volume_upload_intensity(rmd_volume_t *v, const float *host_intensity, const float *host_weight);
+
 /* ---------------------------------------------------------- device image */
 
 /* DeviceImage<T>(width,height) = cudaMallocPitch, device_image.cuh:37-50 */

@@ -86,6 +86,13 @@ _SIGNATURES = {
     "rmd_volume_raycast": (ci, [vp, ci, ci, cf, cf, cf, cf, vp, vp, cs]),
     "rmd_volume_download": (ci, [vp, vp, vp]),
     "rmd_volume_upload": (ci, [vp, vp, vp]),
+    "rmd_volume_enable_intensity": (ci, [vp]),
+    "rmd_volume_integrate_depth_intensity": (ci, [vp, ci, ci, cf, cf, cf, cf, vp, vp, cs, vp, cs, vp, cs]),
+    "rmd_volume_surface_intensity": (ci, [vp, vp, cs, P(cs)]),
+    "rmd_volume_surface_intensity_device": (ci, [vp, vp, cs, P(cs)]),
+    "rmd_volume_raycast_intensity": (ci, [vp, ci, ci, cf, cf, cf, cf, vp, vp, cs, vp, cs]),
+    "rmd_volume_download_intensity": (ci, [vp, vp, vp]),
+    "rmd_volume_upload_intensity": (ci, [vp, vp, vp]),
     "rmd_reduce_sum_f32":(ci, [vp, cs, cs, cs, P(cf)]),
     "rmd_reduce_sum_i32": (ci, [vp, cs, cs, cs, P(ctypes.c_int32)]),
     "rmd_reduce_count_eq_i32": (ci, [vp, cs, cs, cs, ctypes.c_int32, P(cs)]),

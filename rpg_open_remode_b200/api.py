@@ -504,9 +504,12 @@ class DepthmapDenoiser:
 class TsdfVolume:
     """Dense TSDF voxel grid on one device that fuses finished keyframes (rmd_volume_*, include/rmd_b200.h;
     DESIGN.md 4.8).  dims = (nx, ny, nz), x fastest; origin = world position of the centre of voxel (0, 0, 0);
-    truncation in metres; max_weight caps a voxel's weight (one observation = 1)."""
+    truncation in metres; max_weight caps a voxel's weight (one observation = 1).  intensity=True adds the
+    intensity channel (8 B per voxel): keyframes then also fuse their reference image, and the surface points, mesh
+    vertices and raycast views can be shaded (surfaceIntensity, raycastIntensity)."""
 
-    def __init__(self, dims, voxel_size: float, origin, truncation: float, max_weight: float = 64.0, device=-1):
+    def __init__(self, dims, voxel_size: float, origin, truncation: float, max_weight: float = 64.0, device=-1,
+                 intensity: bool = False):
         self.dims = tuple(int(n) for n in dims)
         if len(self.dims) != 3:
             raise ValueError("TsdfVolume: dims must be (nx, ny, nz)")
@@ -518,6 +521,9 @@ class TsdfVolume:
         self._h = h
         self.voxel_size, self.origin = float(_f32(voxel_size)), o.copy()
         self.truncation, self.max_weight = float(_f32(truncation)), float(_f32(max_weight))
+        self.intensity = False
+        if intensity:
+            self.enableIntensity()
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -534,9 +540,15 @@ class TsdfVolume:
         ptr, pitch = (depth.data, depth.pitch) if depth is not None else (None, 0)
         check(self._L.rmd_volume_integrate_seeds(self._h, seeds.handle, ptr, pitch), "TsdfVolume::integrate")
 
-    def integrateDepth(self, depth, cam: PinholeCamera, T_curr_world, conv=None) -> None:
+    def enableIntensity(self) -> None:
+        """Allocate and zero the intensity channel (no-op when it exists)."""
+        check(self._L.rmd_volume_enable_intensity(self._h), "TsdfVolume::enableIntensity")
+        self.intensity = True
+
+    def integrateDepth(self, depth, cam: PinholeCamera, T_curr_world, conv=None, intensity=None) -> None:
         """Any depth image (distance along the ray): a float32 DeviceImage or a host array; conv: optional int32
-        states (DeviceImage or host array), only CONVERGED pixels count."""
+        states (DeviceImage or host array), only CONVERGED pixels count; intensity: optional float32 image of the
+        same size (DeviceImage or host array) fused into the intensity channel."""
         keep = []
 
         def dev(img, dtype):
@@ -552,10 +564,18 @@ class TsdfVolume:
         C = dev(conv, np.int32) if conv is not None else None
         if C is not None and (C.width, C.height) != (D.width, D.height):
             raise ValueError("TsdfVolume::integrateDepth: depth and state maps differ in size")
+        I = dev(intensity, np.float32) if intensity is not None else None
+        if I is not None and (I.width, I.height) != (D.width, D.height):
+            raise ValueError("TsdfVolume::integrateDepth: depth and intensity images differ in size")
         T = _pose12(T_curr_world)
-        check(self._L.rmd_volume_integrate_depth(self._h, D.width, D.height, cam.fx, cam.fy, cam.cx, cam.cy,
-                                                 T.ctypes.data, D.data, D.pitch, C.data if C else None,
-                                                 C.pitch if C else 0), "TsdfVolume::integrateDepth")
+        if I is None:
+            check(self._L.rmd_volume_integrate_depth(self._h, D.width, D.height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                                     T.ctypes.data, D.data, D.pitch, C.data if C else None,
+                                                     C.pitch if C else 0), "TsdfVolume::integrateDepth")
+        else:
+            check(self._L.rmd_volume_integrate_depth_intensity(
+                self._h, D.width, D.height, cam.fx, cam.fy, cam.cx, cam.cy, T.ctypes.data, D.data, D.pitch,
+                C.data if C else None, C.pitch if C else 0, I.data, I.pitch), "TsdfVolume::integrateDepth")
         if keep:
             self.sync()   # the staged images must outlive the kernel
 
@@ -569,6 +589,19 @@ class TsdfVolume:
         out = np.empty((int(capacity), 4), np.float32)
         check(self._L.rmd_volume_surface_points(self._h, out.ctypes.data if capacity else None, int(capacity),
                                                 ctypes.byref(n)), "TsdfVolume::surfacePoints")
+        return out[:min(int(capacity), n.value)]
+
+    def surfaceIntensity(self, capacity: "int | None" = None) -> np.ndarray:
+        """float32 [n]: the intensity of every surface point (and mesh vertex), in surfacePoints() order; -1 where
+        neither of the point's voxels has one.  With a capacity, at most that many."""
+        n = ctypes.c_size_t()
+        if capacity is None:
+            check(self._L.rmd_volume_surface_intensity(self._h, None, 0, ctypes.byref(n)),
+                  "TsdfVolume::surfaceIntensity")
+            capacity = n.value
+        out = np.empty(int(capacity), np.float32)
+        check(self._L.rmd_volume_surface_intensity(self._h, out.ctypes.data if capacity else None, int(capacity),
+                                                   ctypes.byref(n)), "TsdfVolume::surfaceIntensity")
         return out[:min(int(capacity), n.value)]
 
     def mesh(self, vertex_capacity: "int | None" = None, triangle_capacity: "int | None" = None):
@@ -598,6 +631,17 @@ class TsdfVolume:
         self.sync()
         return img.getDevData()
 
+    def raycastIntensity(self, cam: PinholeCamera, T_curr_world, width: int, height: int):
+        """(depth, intensity), float32 [height, width] each: raycast()'s depth, bit for bit, and the fused intensity
+        at each hit, -1 where there is no hit or no intensity."""
+        img, inten = DeviceImage(width, height, "float32"), DeviceImage(width, height, "float32")
+        T = _pose12(T_curr_world)
+        check(self._L.rmd_volume_raycast_intensity(self._h, int(width), int(height), cam.fx, cam.fy, cam.cx, cam.cy,
+                                                   T.ctypes.data, img.data, img.pitch, inten.data, inten.pitch),
+              "TsdfVolume::raycastIntensity")
+        self.sync()
+        return img.getDevData(), inten.getDevData()
+
     def download(self):
         """(tsdf, weight), float32 arrays of shape (nz, ny, nx)."""
         nx, ny, nz = self.dims
@@ -612,6 +656,22 @@ class TsdfVolume:
             raise ValueError("TsdfVolume::upload: wrong size")
         check(self._L.rmd_volume_upload(self._h, t.ctypes.data, w.ctypes.data), "TsdfVolume::upload")
 
+    def downloadIntensity(self):
+        """(intensity, intensity weight), float32 arrays of shape (nz, ny, nx)."""
+        nx, ny, nz = self.dims
+        c, w = np.empty((nz, ny, nx), np.float32), np.empty((nz, ny, nx), np.float32)
+        check(self._L.rmd_volume_download_intensity(self._h, c.ctypes.data, w.ctypes.data),
+              "TsdfVolume::downloadIntensity")
+        return c, w
+
+    def uploadIntensity(self, intensity, weight) -> None:
+        nx, ny, nz = self.dims
+        c, w = (np.ascontiguousarray(a, np.float32) for a in (intensity, weight))
+        if c.size != nx * ny * nz or w.size != nx * ny * nz:
+            raise ValueError("TsdfVolume::uploadIntensity: wrong size")
+        check(self._L.rmd_volume_upload_intensity(self._h, c.ctypes.data, w.ctypes.data),
+              "TsdfVolume::uploadIntensity")
+
     def reset(self) -> None:
         check(self._L.rmd_volume_reset(self._h), "TsdfVolume::reset")
 
@@ -622,16 +682,30 @@ class TsdfVolume:
         check(self._L.rmd_volume_sync(self._h), "TsdfVolume::sync")
 
 
-def write_ply(path: str, vertices, triangles) -> None:
+def write_ply(path: str, vertices, triangles, intensity=None) -> None:
     """Binary little-endian PLY of a mesh such as TsdfVolume.mesh() returns: per vertex float x, y, z and the
-    weight as float `weight`; per face a uchar-counted int list `vertex_indices`."""
+    weight as float `weight`; per face a uchar-counted int list `vertex_indices`.  With `intensity` (one value per
+    vertex in [0, 1], e.g. TsdfVolume.surfaceIntensity()), each vertex also gets uchar red, green, blue =
+    clip(rint(255 i), 0, 255); -1 (no intensity) is written as 0."""
     v = np.ascontiguousarray(vertices, "<f4").reshape(-1, 4)
     t = np.ascontiguousarray(triangles, "<i4").reshape(-1, 3)
     faces = np.empty(len(t), np.dtype([("n", "u1"), ("i", "<i4", 3)]))
     faces["n"], faces["i"] = 3, t
+    colour = ""
+    if intensity is not None:
+        i = np.asarray(intensity, np.float32).reshape(-1)
+        if len(i) != len(v):
+            raise ValueError("write_ply: one intensity per vertex")
+        with np.errstate(invalid="ignore"):
+            g = np.clip(np.rint(np.float32(255) * i), 0, 255)
+        g = np.where(np.isfinite(g), g, 0).astype(np.uint8)
+        rec = np.empty(len(v), np.dtype([("p", "<f4", 4), ("c", "u1", 3)]))
+        rec["p"], rec["c"] = v, g[:, None]
+        v = rec
+        colour = "property uchar red\nproperty uchar green\nproperty uchar blue\n"
     header = ("ply\nformat binary_little_endian 1.0\n"
               "element vertex %d\nproperty float x\nproperty float y\nproperty float z\nproperty float weight\n"
-              "element face %d\nproperty list uchar int vertex_indices\nend_header\n" % (len(v), len(t)))
+              "%selement face %d\nproperty list uchar int vertex_indices\nend_header\n" % (len(v), colour, len(t)))
     with open(path, "wb") as f:
         f.write(header.encode("ascii"))
         f.write(v.tobytes())

@@ -1035,6 +1035,11 @@ int rmd_seeds_set_reference(rmd_seeds_t *s, const float *host_img, const float *
 {
   RMD_REQUIRE(s && host_img && T_curr_world, "rmd_seeds_set_reference: null argument");
   DeviceGuard guard(s->device);
+  {
+    // s->ref may still be read by work another handle enqueued against s (rmd_volume_integrate_seeds)
+    const int rc = wait_external(s);
+    if(rc) return rc;
+  }
   const size_t row = sizeof(float) * (size_t)s->width;
   // pageable source: returns once the data is staged, buffer reusable
   RMD_CUDA_TRY(cudaMemcpy2DAsync(s->ref, s->ref_pitch, host_img, row, row, s->height,
@@ -1049,6 +1054,10 @@ int rmd_seeds_set_reference_device(rmd_seeds_t *s, const float *dev_img, size_t 
   DeviceGuard guard(s->device);
   const size_t row = sizeof(float) * (size_t)s->width;
   RMD_REQUIRE(pitch_bytes >= row, "rmd_seeds_set_reference_device: pitch smaller than a row");
+  {
+    const int rc = wait_external(s);   // as rmd_seeds_set_reference
+    if(rc) return rc;
+  }
   RMD_CUDA_TRY(cudaMemcpy2DAsync(s->ref, s->ref_pitch, dev_img, pitch_bytes, row, s->height,
                                  cudaMemcpyDeviceToDevice, s->stream));
   return finish_set_reference(s, T_curr_world, min_depth, max_depth);
@@ -1059,6 +1068,10 @@ int rmd_seeds_set_reference_u8(rmd_seeds_t *s, const uint8_t *host_img, const fl
 {
   RMD_REQUIRE(s && host_img && T_curr_world, "rmd_seeds_set_reference_u8: null argument");
   DeviceGuard guard(s->device);
+  {
+    const int rc = wait_external(s);   // as rmd_seeds_set_reference
+    if(rc) return rc;
+  }
   // own scratch image: the ring slots belong to frames that may still be in flight
   if(!s->ref_u8)
     RMD_CUDA_TRY(cudaMallocPitch(&s->ref_u8, &s->ref_u8_pitch, (size_t)s->width, s->height));
@@ -2095,6 +2108,10 @@ struct rmd_volume
   unsigned long long *tri_offsets, *tri_total;
   unsigned long long *keys; size_t keys_cap;
   int *tri_stage; size_t tri_stage_cap;
+  // intensity channel (rmd_volume_enable_intensity; NULL = off): n_vox float2 (intensity, weight), indexed like
+  // g.vox, and the host variant's staging of the surface intensities, grown on demand
+  float2 *col;
+  float *istage; size_t istage_cap;
   uint64_t n_total;
 };
 
@@ -2109,8 +2126,10 @@ bool depth_pitch_ok(size_t pitch, int width)
   return pitch >= sizeof(float) * (size_t)width && pitch % sizeof(float) == 0;
 }
 
+// intensity (NULL = the tsdf only): an image of the depth's size, fused into v->col
 int volume_integrate(rmd_volume *v, int width, int height, const Camera &cam, const Pose &T_curr_world,
-                     const float *depth, size_t depth_stride, int depth_comps, const int32_t *conv, size_t conv_stride)
+                     const float *depth, size_t depth_stride, int depth_comps, const int32_t *conv, size_t conv_stride,
+                     const float *intensity = NULL, size_t intensity_stride = 0)
 {
   VolumeIntegrateParams P;
   memset(&P, 0, sizeof(P));
@@ -2121,6 +2140,11 @@ int volume_integrate(rmd_volume *v, int width, int height, const Camera &cam, co
   P.depth = depth; P.depth_stride = depth_stride; P.depth_comps = depth_comps;
   P.conv = conv; P.conv_stride = conv_stride;
   P.trunc = v->trunc; P.max_weight = v->max_weight;
+  if(intensity)
+  {
+    P.col = v->col;
+    P.intensity = intensity; P.intensity_stride = intensity_stride;
+  }
   RMD_CUDA_TRY(launch_volume_integrate(P, v->stream));
   v->n_total += 1;
   return 0;
@@ -2311,6 +2335,7 @@ int rmd_volume_destroy(rmd_volume_t *v)
   cudaFree(v->g.vox);
   cudaFree(v->surf_offsets); cudaFree(v->surf_total); cudaFree(v->stage);
   cudaFree(v->tri_offsets); cudaFree(v->tri_total); cudaFree(v->keys); cudaFree(v->tri_stage);
+  cudaFree(v->col); cudaFree(v->istage);
   cudaGetLastError();
   delete v;
   return 0;
@@ -2330,6 +2355,8 @@ int rmd_volume_reset(rmd_volume_t *v)
   RMD_REQUIRE(v, "rmd_volume_reset: null handle");
   DeviceGuard guard(v->device);
   RMD_CUDA_TRY(cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->stream));
+  if(v->col)
+    RMD_CUDA_TRY(cudaMemsetAsync(v->col, 0, sizeof(float2) * v->n_vox, v->stream));
   return 0;
 }
 
@@ -2366,11 +2393,14 @@ int rmd_volume_integrate_seeds(rmd_volume_t *v, rmd_seeds_t *s, const float *dev
   RMD_CUDA_TRY(cudaStreamWaitEvent(v->stream, v->seeds_ev, 0));
   if(s->ext_pending)
     RMD_CUDA_TRY(cudaStreamWaitEvent(v->stream, s->ext_ev, 0));
+  // with the intensity channel, the reference image is fused too
+  const float *ref = v->col ? s->ref : NULL;
+  const size_t ref_stride = s->ref_pitch / sizeof(float);
   const int rc = dev_depth
       ? volume_integrate(v, s->width, s->height, s->cam, s->T_ref_world, dev_depth, depth_pitch / sizeof(float), 1,
-                         s->conv, s->conv_pitch / sizeof(int))
+                         s->conv, s->conv_pitch / sizeof(int), ref, ref_stride)
       : volume_integrate(v, s->width, s->height, s->cam, s->T_ref_world, reinterpret_cast<const float*>(s->seed),
-                         (size_t)s->seed_stride * 4, 4, s->conv, s->conv_pitch / sizeof(int));
+                         (size_t)s->seed_stride * 4, 4, s->conv, s->conv_pitch / sizeof(int), ref, ref_stride);
   if(rc) return rc;
   // ... and a later writer of the seeds (update, set_reference, upload_state) waits for the kernel's reads
   RMD_CUDA_TRY(cudaEventRecord(s->ext_ev, v->stream));
@@ -2522,6 +2552,186 @@ int rmd_volume_upload(rmd_volume_t *v, const float *host_tsdf, const float *host
     for(size_t q = 0; q < m; ++q)
       tmp[q] = make_float2(host_tsdf[b + q], host_weight[b + q]);
     err = cudaMemcpyAsync(v->g.vox + b, tmp, sizeof(float2) * m, cudaMemcpyHostToDevice, v->stream);
+    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);   // tmp is refilled next
+  }
+  free(tmp);
+  RMD_CUDA_TRY(err);
+  return 0;
+}
+
+} // extern "C"
+
+// ============================================================ TSDF volume: intensity channel
+
+namespace
+{
+
+// Surface intensities: the surface points' count pass and scan, then their write pass in its intensity instance
+// (same blocks, same ranks).  host: min(count, capacity) are staged in v->istage and copied to out.  Synchronous.
+int volume_surface_intensity(rmd_volume *v, float *out, size_t capacity, size_t *count, bool host)
+{
+  VolumeSurfaceParams P;
+  {
+    const int rc = volume_surface_count(v, P, count);
+    if(rc) return rc;
+  }
+  const size_t n = *count < capacity ? *count : capacity;
+  if(!n)
+    return 0;
+  if(host)
+  {
+    const int rc = volume_grow(&v->istage, &v->istage_cap, n);
+    if(rc) return rc;
+  }
+  P.col = v->col;
+  P.intensity = host ? v->istage : out;
+  P.capacity = n;
+  RMD_CUDA_TRY(launch_volume_surface_write_intensity(P, v->stream));
+  v->n_total += 1;
+  if(host)
+    RMD_CUDA_TRY(cudaMemcpyAsync(out, v->istage, n * sizeof(float), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  return 0;
+}
+
+int no_intensity(const char *what)
+{
+  return fail(RMD_ERR_NOT_INITIALISED, (std::string(what) + ": the volume has no intensity channel").c_str());
+}
+
+} // namespace
+
+extern "C"
+{
+
+int rmd_volume_enable_intensity(rmd_volume_t *v)
+{
+  RMD_REQUIRE(v, "rmd_volume_enable_intensity: null handle");
+  if(v->col)
+    return 0;
+  DeviceGuard guard(v->device);
+  cudaError_t err = cudaMalloc(&v->col, sizeof(float2) * v->n_vox);
+  if(err != cudaSuccess)
+  {
+    v->col = NULL;
+    return fail_cuda(err, "rmd_volume_enable_intensity");
+  }
+  err = cudaMemsetAsync(v->col, 0, sizeof(float2) * v->n_vox, v->stream);
+  if(err != cudaSuccess)
+  {
+    cudaFree(v->col);
+    v->col = NULL;
+    return fail_cuda(err, "rmd_volume_enable_intensity");
+  }
+  return 0;
+}
+
+int rmd_volume_integrate_depth_intensity(rmd_volume_t *v, int width, int height, float fx, float fy, float cx,
+                                         float cy, const float *T_curr_world, const float *dev_depth,
+                                         size_t depth_pitch, const int32_t *dev_conv, size_t conv_pitch,
+                                         const float *dev_intensity, size_t intensity_pitch)
+{
+  RMD_REQUIRE(v && T_curr_world && dev_depth && dev_intensity, "rmd_volume_integrate_depth_intensity: null argument");
+  RMD_REQUIRE(width > 0 && height > 0, "rmd_volume_integrate_depth_intensity: bad image size");
+  RMD_REQUIRE(depth_pitch_ok(depth_pitch, width), "rmd_volume_integrate_depth_intensity: bad depth pitch");
+  RMD_REQUIRE(!dev_conv || (conv_pitch >= sizeof(int32_t) * (size_t)width && conv_pitch % sizeof(int32_t) == 0),
+              "rmd_volume_integrate_depth_intensity: bad state pitch");
+  RMD_REQUIRE(depth_pitch_ok(intensity_pitch, width), "rmd_volume_integrate_depth_intensity: bad intensity pitch");
+  if(!v->col)
+    return no_intensity("rmd_volume_integrate_depth_intensity");
+  DeviceGuard guard(v->device);
+  Camera cam;
+  cam.fx = fx; cam.fy = fy; cam.cx = cx; cam.cy = cy;
+  return volume_integrate(v, width, height, cam, pose_from(T_curr_world), dev_depth, depth_pitch / sizeof(float), 1,
+                          dev_conv, conv_pitch / sizeof(int32_t), dev_intensity, intensity_pitch / sizeof(float));
+}
+
+int rmd_volume_surface_intensity(rmd_volume_t *v, float *host_intensity, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (host_intensity || capacity == 0), "rmd_volume_surface_intensity: null argument");
+  if(!v->col)
+    return no_intensity("rmd_volume_surface_intensity");
+  DeviceGuard guard(v->device);
+  return volume_surface_intensity(v, host_intensity, capacity, count, true);
+}
+
+int rmd_volume_surface_intensity_device(rmd_volume_t *v, float *dev_intensity, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (dev_intensity || capacity == 0), "rmd_volume_surface_intensity_device: null argument");
+  RMD_REQUIRE(((uintptr_t)dev_intensity % 4) == 0, "rmd_volume_surface_intensity_device: output must be 4-byte aligned");
+  if(!v->col)
+    return no_intensity("rmd_volume_surface_intensity_device");
+  DeviceGuard guard(v->device);
+  return volume_surface_intensity(v, dev_intensity, capacity, count, false);
+}
+
+int rmd_volume_raycast_intensity(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                                 const float *T_curr_world, float *dev_depth, size_t depth_pitch,
+                                 float *dev_intensity, size_t intensity_pitch)
+{
+  RMD_REQUIRE(v && T_curr_world && dev_depth && dev_intensity, "rmd_volume_raycast_intensity: null argument");
+  RMD_REQUIRE(width > 0 && height > 0, "rmd_volume_raycast_intensity: bad image size");
+  RMD_REQUIRE(depth_pitch_ok(depth_pitch, width), "rmd_volume_raycast_intensity: bad depth pitch");
+  RMD_REQUIRE(depth_pitch_ok(intensity_pitch, width), "rmd_volume_raycast_intensity: bad intensity pitch");
+  if(!v->col)
+    return no_intensity("rmd_volume_raycast_intensity");
+  DeviceGuard guard(v->device);
+  VolumeRaycastIntensityParams P;
+  memset(&P, 0, sizeof(P));
+  P.r.g = v->g;
+  P.r.width = width; P.r.height = height;
+  P.r.cam.fx = fx; P.r.cam.fy = fy; P.r.cam.cx = cx; P.r.cam.cy = cy;
+  P.r.T_world_curr = pose_inverse(pose_from(T_curr_world));
+  P.r.depth = dev_depth; P.r.depth_stride = depth_pitch / sizeof(float);
+  P.col = v->col;
+  P.intensity = dev_intensity; P.intensity_stride = intensity_pitch / sizeof(float);
+  RMD_CUDA_TRY(launch_volume_raycast_intensity(P, v->stream));
+  v->n_total += 1;
+  return 0;
+}
+
+int rmd_volume_download_intensity(rmd_volume_t *v, float *host_intensity, float *host_weight)
+{
+  RMD_REQUIRE(v && host_intensity && host_weight, "rmd_volume_download_intensity: null argument");
+  if(!v->col)
+    return no_intensity("rmd_volume_download_intensity");
+  DeviceGuard guard(v->device);
+  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
+  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
+  if(!tmp) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_download_intensity: host allocation failed");
+  cudaError_t err = cudaSuccess;
+  for(size_t b = 0; b < v->n_vox && err == cudaSuccess; b += chunk)
+  {
+    const size_t m = v->n_vox - b < chunk ? v->n_vox - b : chunk;
+    err = cudaMemcpyAsync(tmp, v->col + b, sizeof(float2) * m, cudaMemcpyDeviceToHost, v->stream);
+    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);
+    for(size_t q = 0; q < m && err == cudaSuccess; ++q)
+    {
+      host_intensity[b + q] = tmp[q].x;
+      host_weight[b + q] = tmp[q].y;
+    }
+  }
+  free(tmp);
+  RMD_CUDA_TRY(err);
+  return 0;
+}
+
+int rmd_volume_upload_intensity(rmd_volume_t *v, const float *host_intensity, const float *host_weight)
+{
+  RMD_REQUIRE(v && host_intensity && host_weight, "rmd_volume_upload_intensity: null argument");
+  if(!v->col)
+    return no_intensity("rmd_volume_upload_intensity");
+  DeviceGuard guard(v->device);
+  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
+  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
+  if(!tmp) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_upload_intensity: host allocation failed");
+  cudaError_t err = cudaSuccess;
+  for(size_t b = 0; b < v->n_vox && err == cudaSuccess; b += chunk)
+  {
+    const size_t m = v->n_vox - b < chunk ? v->n_vox - b : chunk;
+    for(size_t q = 0; q < m; ++q)
+      tmp[q] = make_float2(host_intensity[b + q], host_weight[b + q]);
+    err = cudaMemcpyAsync(v->col + b, tmp, sizeof(float2) * m, cudaMemcpyHostToDevice, v->stream);
     if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);   // tmp is refilled next
   }
   free(tmp);

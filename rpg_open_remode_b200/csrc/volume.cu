@@ -18,8 +18,21 @@ __device__ __forceinline__ float voxel_coord(float origin, int i, float s)
   return __fadd_rn(origin, __fmul_rn((float)i, s));
 }
 
+__device__ __forceinline__ bool finite_f(float a)
+{
+  return (__float_as_uint(a) & 0x7f800000u) != 0x7f800000u;
+}
+
+__device__ __forceinline__ float lerp_rn(float a, float b, float f)
+{
+  return __fadd_rn(a, __fmul_rn(f, __fsub_rn(b, a)));
+}
+
 // One thread per voxel, x fastest, so that the float2 records of a warp are contiguous.  The frustum and depth
-// tests come before the record is loaded: a voxel outside the image costs no memory traffic.
+// tests come before the record is loaded: a voxel outside the image costs no memory traffic.  INTENSITY: then a
+// voxel in the band (sdf < tau) also averages the intensity at its pixel into its colour record; the condition
+// does not depend on the tsdf record, and a voxel outside the band loads no colour record.
+template<bool INTENSITY>
 __global__ void __launch_bounds__(256) volume_integrate_kernel(const VolumeIntegrateParams P)
 {
   const VolumeGrid &g = P.g;
@@ -61,6 +74,16 @@ __global__ void __launch_bounds__(256) volume_integrate_kernel(const VolumeInteg
   const float w1 = __fadd_rn(rec.y, 1.0f);
   const float t1 = __fdiv_rn(__fadd_rn(__fmul_rn(rec.x, rec.y), o), w1);
   g.vox[lin] = make_float2(t1, fminf(w1, P.max_weight));
+  if(INTENSITY && sdf < P.trunc)
+  {
+    const float I = P.intensity[(size_t)y * P.intensity_stride + x];
+    if(!finite_f(I))
+      return;
+    const float2 c = P.col[lin];
+    const float wc1 = __fadd_rn(c.y, 1.0f);
+    const float c1 = __fdiv_rn(__fadd_rn(__fmul_rn(c.x, c.y), I), wc1);
+    P.col[lin] = make_float2(c1, fminf(wc1, P.max_weight));
+  }
 }
 
 // ---------------------------------------------------------------------------------------- surface points
@@ -128,6 +151,18 @@ __device__ __forceinline__ float4 surface_point(const VolumeGrid &g, const Surfa
   else o.z = __fadd_rn(o.z, step);
   o.w = fminf(c.a.y, b.y);
   return o;
+}
+
+// Intensity of the point of voxel n on `axis`: the colour records of its two voxels, interpolated with the
+// position's factor t_a / (t_a - t_b) when both are known.
+__device__ __forceinline__ float surface_intensity(const VolumeSurfaceParams &P, const SurfaceCell &c, unsigned int n,
+                                                   int axis)
+{
+  const size_t step = axis == 0 ? (size_t)1 : axis == 1 ? (size_t)P.g.nx : (size_t)P.g.nx * (size_t)P.g.ny;
+  const float2 ca = __ldg(P.col + n), cb = __ldg(P.col + (size_t)n + step);
+  if(ca.y > 0.0f && cb.y > 0.0f)
+    return lerp_rn(ca.x, cb.x, __fdiv_rn(c.a.x, __fsub_rn(c.a.x, c.b[axis].x)));
+  return ca.y > 0.0f ? ca.x : cb.y > 0.0f ? cb.x : -1.0f;
 }
 
 __device__ __forceinline__ unsigned int grid_voxels(const VolumeGrid &g)
@@ -219,7 +254,8 @@ __global__ void __launch_bounds__(VOLUME_SCAN_BLOCK) volume_surface_scan_kernel(
 }
 
 // KEYS (the mesh path): also write every point's key 3 * voxel + axis, for all *total points whatever the capacity.
-template<bool KEYS>
+// INTENSITY: write every point's intensity to P.intensity instead of its position to P.out.
+template<bool KEYS, bool INTENSITY>
 __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_write_kernel(const VolumeSurfaceParams P)
 {
   __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
@@ -256,7 +292,12 @@ __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_write_kernel
       if(!(c.mask & (1u << axis)))
         continue;
       if(slot < P.capacity)
-        P.out[slot] = surface_point(P.g, c, axis);
+      {
+        if(INTENSITY)
+          P.intensity[slot] = surface_intensity(P, c, base + r * VOLUME_SURF_BLOCK, axis);
+        else
+          P.out[slot] = surface_point(P.g, c, axis);
+      }
       if(KEYS)
         P.keys[slot] = 3ull * (base + r * VOLUME_SURF_BLOCK) + axis;
       ++slot;
@@ -393,9 +434,28 @@ __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_mesh_write_kernel(co
 }
 
 // --------------------------------------------------------------------------------------------- raycast
-__device__ __forceinline__ float lerp_rn(float a, float b, float f)
+// Trilinear intensity at grid coordinates (gx, gy, gz), interpolated in x, then y, then z; -1 if a corner lies
+// outside the grid or has colour weight 0.
+__device__ __forceinline__ float sample_intensity(const VolumeGrid &g, const float2 *col, float gx, float gy, float gz)
 {
-  return __fadd_rn(a, __fmul_rn(f, __fsub_rn(b, a)));
+  const float x0 = floorf(gx), y0 = floorf(gy), z0 = floorf(gz);
+  const int i0 = (x0 >= 0.0f && x0 < 2.0e9f) ? (int)x0 : -1;
+  const int j0 = (y0 >= 0.0f && y0 < 2.0e9f) ? (int)y0 : -1;
+  const int k0 = (z0 >= 0.0f && z0 < 2.0e9f) ? (int)z0 : -1;
+  if(i0 < 0 || j0 < 0 || k0 < 0 || i0 + 1 >= g.nx || j0 + 1 >= g.ny || k0 + 1 >= g.nz)
+    return -1.0f;
+  const size_t plane = (size_t)g.nx * g.ny;
+  const float2 *b = col + ((size_t)k0 * g.ny + j0) * g.nx + i0;
+  const float2 c000 = __ldg(b), c100 = __ldg(b + 1), c010 = __ldg(b + g.nx), c110 = __ldg(b + g.nx + 1);
+  const float2 c001 = __ldg(b + plane), c101 = __ldg(b + plane + 1), c011 = __ldg(b + plane + g.nx),
+               c111 = __ldg(b + plane + g.nx + 1);
+  if(c000.y == 0.0f || c100.y == 0.0f || c010.y == 0.0f || c110.y == 0.0f || c001.y == 0.0f || c101.y == 0.0f ||
+     c011.y == 0.0f || c111.y == 0.0f)
+    return -1.0f;
+  const float fx = __fsub_rn(gx, x0), fy = __fsub_rn(gy, y0), fz = __fsub_rn(gz, z0);
+  const float c00 = lerp_rn(c000.x, c100.x, fx), c10 = lerp_rn(c010.x, c110.x, fx);
+  const float c01 = lerp_rn(c001.x, c101.x, fx), c11 = lerp_rn(c011.x, c111.x, fx);
+  return lerp_rn(lerp_rn(c00, c10, fy), lerp_rn(c01, c11, fy), fz);
 }
 
 // Trilinear TSDF at grid coordinates (gx, gy, gz); false if a corner lies outside the grid or is unknown.
@@ -422,12 +482,12 @@ __device__ __forceinline__ bool sample_tsdf(const VolumeGrid &g, float gx, float
   return true;
 }
 
-__global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycastParams P)
+// The ray of pixel (x, y).  INTENSITY: also the intensity at the hit, from the grid coordinates of org + t dir in the
+// march's form, into I (the plain instance ignores col and I).
+template<bool INTENSITY>
+__device__ __forceinline__ void raycast_pixel(const VolumeRaycastParams &P, int x, int y, const float2 *col, float *I,
+                                              size_t I_stride)
 {
-  const int x = blockIdx.x * blockDim.x + threadIdx.x;
-  const int y = blockIdx.y * blockDim.y + threadIdx.y;
-  if(x >= P.width || y >= P.height)
-    return;
   const VolumeGrid &g = P.g;
   // the ray of back_project (point_cloud.cuh), rotated into the world; it starts at the camera centre
   const float vx = __fdiv_rn(__fsub_rn((float)x, P.cam.cx), P.cam.fx);
@@ -459,7 +519,7 @@ __global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycast
     t0 = fmaxf(t0, fminf(ta, tb));
     t1 = fminf(t1, fmaxf(ta, tb));
   }
-  float out = 0.0f;
+  float out = 0.0f, inten = -1.0f;
   if(inside && t0 <= t1)
   {
     // a segment inside the box is at most nx + ny + nz voxels long: the bound only stops a ray whose steps
@@ -481,6 +541,10 @@ __global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycast
       if(known && prev_known && f_prev > 0.0f && f <= 0.0f)
       {
         out = __fadd_rn(t_prev, __fdiv_rn(__fmul_rn(s, f_prev), __fsub_rn(f_prev, f)));
+        if(INTENSITY)
+          inten = sample_intensity(g, col, __fdiv_rn(__fsub_rn(__fadd_rn(org[0], __fmul_rn(out, dir[0])), g.ox), s),
+                                   __fdiv_rn(__fsub_rn(__fadd_rn(org[1], __fmul_rn(out, dir[1])), g.oy), s),
+                                   __fdiv_rn(__fsub_rn(__fadd_rn(org[2], __fmul_rn(out, dir[2])), g.oz), s));
         break;
       }
       prev_known = known;
@@ -489,6 +553,26 @@ __global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycast
     }
   }
   P.depth[(size_t)y * P.depth_stride + x] = out;
+  if(INTENSITY)
+    I[(size_t)y * I_stride + x] = inten;
+}
+
+__global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycastParams P)
+{
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const int y = blockIdx.y * blockDim.y + threadIdx.y;
+  if(x >= P.width || y >= P.height)
+    return;
+  raycast_pixel<false>(P, x, y, nullptr, nullptr, 0);
+}
+
+__global__ void __launch_bounds__(256) volume_raycast_intensity_kernel(const VolumeRaycastIntensityParams P)
+{
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const int y = blockIdx.y * blockDim.y + threadIdx.y;
+  if(x >= P.r.width || y >= P.r.height)
+    return;
+  raycast_pixel<true>(P.r, x, y, P.col, P.intensity, P.intensity_stride);
 }
 
 } // namespace
@@ -496,7 +580,10 @@ __global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycast
 cudaError_t launch_volume_integrate(const VolumeIntegrateParams &P, cudaStream_t stream)
 {
   const unsigned int n = (unsigned int)P.g.nx * (unsigned int)P.g.ny * (unsigned int)P.g.nz;
-  volume_integrate_kernel<<<(n + 255u) / 256u, 256, 0, stream>>>(P);
+  if(P.col)
+    volume_integrate_kernel<true><<<(n + 255u) / 256u, 256, 0, stream>>>(P);
+  else
+    volume_integrate_kernel<false><<<(n + 255u) / 256u, 256, 0, stream>>>(P);
   return cudaGetLastError();
 }
 
@@ -511,13 +598,19 @@ cudaError_t launch_volume_surface_count(const VolumeSurfaceParams &P, cudaStream
 
 cudaError_t launch_volume_surface_write(const VolumeSurfaceParams &P, cudaStream_t stream)
 {
-  volume_surface_write_kernel<false><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  volume_surface_write_kernel<false, false><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   return cudaGetLastError();
 }
 
 cudaError_t launch_volume_surface_write_keys(const VolumeSurfaceParams &P, cudaStream_t stream)
 {
-  volume_surface_write_kernel<true><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  volume_surface_write_kernel<true, false><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_surface_write_intensity(const VolumeSurfaceParams &P, cudaStream_t stream)
+{
+  volume_surface_write_kernel<false, true><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   return cudaGetLastError();
 }
 
@@ -547,6 +640,14 @@ cudaError_t launch_volume_raycast(const VolumeRaycastParams &P, cudaStream_t str
   const dim3 block(32, 8);
   const dim3 grid((P.width + block.x - 1) / block.x, (P.height + block.y - 1) / block.y);
   volume_raycast_kernel<<<grid, block, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_raycast_intensity(const VolumeRaycastIntensityParams &P, cudaStream_t stream)
+{
+  const dim3 block(32, 8);
+  const dim3 grid((P.r.width + block.x - 1) / block.x, (P.r.height + block.y - 1) / block.y);
+  volume_raycast_intensity_kernel<<<grid, block, 0, stream>>>(P);
   return cudaGetLastError();
 }
 

@@ -1,6 +1,7 @@
 """Device time of the TSDF volume's operations (DESIGN.md 4.8, 6) on bench.py's c2 scene (VGA): integration of one
 keyframe's depth and state map into a 256^3 and a 512^3 grid over the scene, surface-point extraction, the
-triangle mesh (rmd_volume_mesh_device, vertices and triangles) and a VGA raycast.  Each time is the median of REPEATS runs after WARMUP, measured with CUDA events on the volume's stream.
+triangle mesh (rmd_volume_mesh_device, vertices and triangles) and a VGA raycast, and the intensity channel's
+variants of integration (the frame's image fused too), surface extraction and raycast next to the plain ones.  Each time is the median of REPEATS runs after WARMUP, measured with CUDA events on the volume's stream.
 The achieved bandwidth of an integration counts 16 B per updated voxel (record read + write) and 8 B per pixel
 (depth + state) over its kernel time, against the 3.35 TB/s of the H100 SXM data sheet.  Prints one JSON line with
 the GPU's name and power limit.  GPU box only."""
@@ -65,13 +66,16 @@ def main():
     conv = rmd.DeviceImage(W, H, "int32")
     conv.setDevData(np.ones((H, W), np.int32))              # every pixel CONVERGED: the state map is read
     out = rmd.DeviceImage(W, H, "float32")
+    image = rmd.DeviceImage(W, H, "float32")
+    image.setDevData(fr.image)
+    out_i = rmd.DeviceImage(W, H, "float32")
     T = np.ascontiguousarray(fr.T_cam_world.reshape(12))
     c = ctypes.c_float
     stream = torch.cuda.Stream()
     result = {}
     for n in GRIDS:
         s = float(np.float32((hi - lo).max() / (n - 1 - 16)))   # tau = 4 voxels, padded by 2 tau
-        v = rmd.TsdfVolume((n, n, n), s, lo - 8 * s, 4 * s, 64.0, device=0)
+        v = rmd.TsdfVolume((n, n, n), s, lo - 8 * s, 4 * s, 64.0, device=0, intensity=True)
         v.setStream(stream.cuda_stream)
 
         def integrate():
@@ -83,6 +87,13 @@ def main():
         updated = int((v.download()[1] > 0).sum())
         v.reset()
         ms_int, runs_int = timed(stream, torch, integrate)
+
+        def integrate_intensity():
+            _native.check(L.rmd_volume_integrate_depth_intensity(
+                v.handle, W, H, c(cam.fx), c(cam.fy), c(cam.cx), c(cam.cy), T.ctypes.data, depth.data, depth.pitch,
+                conv.data, conv.pitch, image.data, image.pitch))
+
+        ms_int_i, runs_int_i = timed(stream, torch, integrate_intensity)
         count = ctypes.c_size_t()
         points = rmd.DeviceImage(4 * 4 * n * n, 1, "float32")   # room for 4 n^2 points
 
@@ -90,6 +101,11 @@ def main():
             _native.check(L.rmd_volume_surface_points_device(v.handle, points.data, 4 * n * n, ctypes.byref(count)))
 
         ms_pts, runs_pts = timed(stream, torch, extract)
+
+        def extract_intensity():
+            _native.check(L.rmd_volume_surface_intensity_device(v.handle, points.data, 4 * n * n, ctypes.byref(count)))
+
+        ms_pts_i, runs_pts_i = timed(stream, torch, extract_intensity)
         n_tri = ctypes.c_size_t()
         tris = rmd.DeviceImage(3 * 8 * n * n, 1, "int32")         # room for 8 n^2 triangles
 
@@ -105,6 +121,12 @@ def main():
                                                T.ctypes.data, out.data, out.pitch))
 
         ms_ray, runs_ray = timed(stream, torch, raycast)
+
+        def raycast_intensity():
+            _native.check(L.rmd_volume_raycast_intensity(v.handle, W, H, c(cam.fx), c(cam.fy), c(cam.cx), c(cam.cy),
+                                                         T.ctypes.data, out.data, out.pitch, out_i.data, out_i.pitch))
+
+        ms_ray_i, runs_ray_i = timed(stream, torch, raycast_intensity)
         v.sync()
         hit = int((out.getDevData() > 0).sum())
         algo_bytes = 16 * updated + 8 * W * H
@@ -119,7 +141,13 @@ def main():
             "surface_points_record_bandwidth_TBps": 8 * n ** 3 / (ms_pts * 1e-3) / 1e12,
             "mesh_vertices": int(count.value), "mesh_triangles": int(n_tri.value), "mesh_ms": ms_mesh,
             "mesh_ms_runs": runs_mesh, "mesh_over_surface_points": ms_mesh / ms_pts,
-            "raycast_vga_ms": ms_ray, "raycast_vga_ms_runs": runs_ray, "raycast_pixels_hit": hit}
+            "raycast_vga_ms": ms_ray, "raycast_vga_ms_runs": runs_ray, "raycast_pixels_hit": hit,
+            "integrate_intensity_ms": ms_int_i, "integrate_intensity_ms_runs": runs_int_i,
+            "integrate_intensity_over_plain": ms_int_i / ms_int,
+            "surface_intensity_ms": ms_pts_i, "surface_intensity_ms_runs": runs_pts_i,
+            "surface_intensity_over_points": ms_pts_i / ms_pts,
+            "raycast_intensity_vga_ms": ms_ray_i, "raycast_intensity_vga_ms_runs": runs_ray_i,
+            "raycast_intensity_over_plain": ms_ray_i / ms_ray}
         del v
     try:
         q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
