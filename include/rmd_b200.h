@@ -125,7 +125,8 @@ enum rmd_seeds_option {
   RMD_OPT_TUNE_WARP_TILE_SEEDS = 17, /* tiles with at most this many seeds to update (and a few dozen candidates) are processed by one warp, eight tiles per CTA (8 = the most; 0 = off) */
   RMD_OPT_TUNE_GRID_CTAS = 18,      /* size of the persistent grid (0, the default: one CTA per resident slot, SMs x occupancy) */
   RMD_OPT_TUNE_CTAS_PER_SM = 19,    /* 5x5 staged kernel: the 128-register build (2, = 0, the default) or the 80-register build (3; sized for 3 CTAs per SM, of which two fit next to the 60 KB strips) */
-  RMD_OPT_TUNE_WARP_TILE_CANDS = 20  /* ... and at most this many candidates in all (64 = the most) */
+  RMD_OPT_TUNE_WARP_TILE_CANDS = 20, /* ... and at most this many candidates in all (64 = the most) */
+  RMD_OPT_TUNE_RUN_CHUNKS = 21       /* 4-candidate chunks one work item of the staged search scores (0, the default: chosen per tile; 1..36) */
 };
 
 typedef struct rmd_seeds rmd_seeds_t;

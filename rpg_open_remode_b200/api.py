@@ -44,6 +44,7 @@ OPT_TUNE_WARP_TILE_SEEDS = 17
 OPT_TUNE_GRID_CTAS = 18
 OPT_TUNE_CTAS_PER_SM = 19
 OPT_TUNE_WARP_TILE_CANDS = 20
+OPT_TUNE_RUN_CHUNKS = 21
 FIELD_DEBUG_TIMELINE = 100
 VARIANT_STAGED, VARIANT_DIRECT = 0, 1
 # sigma^2 of a propagated keyframe prior as a fraction of the uniform prior's range^2 / 36 (DESIGN.md 4.7, 6)

@@ -192,7 +192,7 @@ struct rmd_seeds
   bool worklist_valid;         // false: rebuild (all tiles, image order) before the next staged launch
   bool last_staged;            // the last update ran the staged kernel (retired count applies)
   int tiles_x;
-  int tune[11];                // split_max, split_min_items, split_items_per_cta, sparse_max_seeds, heavy_min_items, split_avg_pct, pdl, warp_tile_max_seeds, grid_ctas, (ctas_per_sm: own field), warp_tile_max_cands
+  int tune[12];                // split_max, split_min_items, split_items_per_cta, sparse_max_seeds, heavy_min_items, split_avg_pct, pdl, warp_tile_max_seeds, grid_ctas, (ctas_per_sm: own field), warp_tile_max_cands, run_chunks
   ParallelCopier *copier;   // host frame -> pinned ring (created on first host update)
   // lens undistortion of 8-bit frames (ingest.cuh); maps are null until init_undistortion_map
   short2 *undist_xy; uint16_t *undist_frac;
@@ -527,6 +527,7 @@ int prepare_update(rmd_seeds *s, const float *curr, size_t curr_pitch, const flo
     P.warp_tile_max_seeds = s->tune[7];
     P.warp_tile_max_cands = s->tune[10];
     P.grid_ctas = s->tune[8];
+    P.run_chunks = s->tune[11];
     P.counts_cur = s->work_counts + 8 * (f % 3);
     P.counts_next = s->work_counts + 8 * ((f + 1) % 3);
     P.counts_zero = s->work_counts + 8 * ((f + 2) % 3);
@@ -928,6 +929,7 @@ int rmd_seeds_create(int width, int height, float fx, float fy, float cx, float 
   s->tune[4] = staged::HEAVY_MIN_ITEMS; s->tune[5] = staged::SPLIT_AVG_PCT; s->tune[6] = 1;
   s->tune[7] = staged::WARP_TILE_MAX_SEEDS;
   s->tune[10] = staged::WARP_TILE_MAX_CANDS;
+  s->tune[11] = 0;
   s->variant = 0;   // staged (the fast path) unless RMD_OPT_KERNEL_VARIANT says otherwise
   s->chain_frames = 1;   // chaining is opt-in (include/rmd_b200.h, RMD_OPT_CHAIN_FRAMES)
   s->seed_mode_pct = 0;   // off by default: measured slower than the tile organisation on the bench workloads (DESIGN.md 4.1c)
@@ -1021,6 +1023,10 @@ int rmd_seeds_set_option(rmd_seeds_t *s, int option, int value)
   case RMD_OPT_TUNE_CTAS_PER_SM:
     RMD_REQUIRE(value == 0 || value == 2 || value == 3, "RMD_OPT_TUNE_CTAS_PER_SM: 0 (automatic), 2 or 3");
     s->ctas_per_sm = value;
+    return 0;
+  case RMD_OPT_TUNE_RUN_CHUNKS:
+    RMD_REQUIRE(value >= 0 && value <= staged::MAX_CHUNKS, "RMD_OPT_TUNE_RUN_CHUNKS: 0 (automatic)..36");
+    s->tune[11] = value;
     return 0;
   case RMD_OPT_TEX_FRAC_BITS:
     RMD_REQUIRE(value >= 0 && value <= 12, "RMD_OPT_TEX_FRAC_BITS: 0..12");

@@ -126,6 +126,7 @@ struct FilterParams
   int warp_tile_max_cands;               // a warp tile has at most this many candidates in all
   int ctas_per_sm;                       // 5x5 staged kernel: 2 (128 registers) or 3 (80 registers) resident CTAs per SM (host side only)
   int grid_ctas;                         // 0: one CTA per resident slot; else the persistent grid's size (host side only)
+  int run_chunks;                        // chunks per work item of the staged search; 0: chosen per tile
   // {heavy entries, light entries, helper entries reserved, work items of the frame, tiles listed (lead
   //  entries), lead CTAs of the previous frame that have finished listing, sparse entries, -}: 8 uints per frame
   const unsigned int *counts_cur;

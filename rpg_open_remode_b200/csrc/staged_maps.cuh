@@ -18,6 +18,14 @@ constexpr int NTHREADS = 32 * NWARPS;
 constexpr int NPIX = TILE_W * TILE_H;  // seeds per CTA
 constexpr int CHUNK = 4;               // candidates per work item
 constexpr int MAX_CHUNKS = 36;         // ceil(143 / CHUNK): 100 px / 0.7 px + 1 = 143 candidates
+#ifndef RMD_RUN_MAX_CHUNKS
+#define RMD_RUN_MAX_CHUNKS 9
+#endif
+#ifndef RMD_RUN_MIN_ROUNDS
+#define RMD_RUN_MIN_ROUNDS 2
+#endif
+constexpr int RUN_MAX_CHUNKS = RMD_RUN_MAX_CHUNKS;  // longest run of chunks one work item scores (automatic choice)
+constexpr int RUN_MIN_ROUNDS = RMD_RUN_MIN_ROUNDS;  // ... while every warp of the tile still gets this many rounds (2: DESIGN.md 4.1)
 #ifndef RMD_STRIP_FLOATS
 #define RMD_STRIP_FLOATS 15360
 #endif

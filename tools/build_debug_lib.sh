@@ -6,9 +6,9 @@ cd "$(dirname "$0")/.."
 mkdir -p tools/build/dbg
 SRC=rpg_open_remode_b200/csrc
 FLAGS="-std=c++17 -O3 -gencode arch=compute_90a,code=sm_90a -lineinfo -use_fast_math -Xcompiler -fPIC -DRMD_DEBUG_COUNTERS=1"
-for f in c_api depth_filter depth_filter_staged denoiser reduction ingest point_cloud; do
-  nvcc $FLAGS -c $SRC/$f.cu -o tools/build/dbg/$f.o &
+for f in $SRC/*.cu; do
+  nvcc $FLAGS -c $f -o tools/build/dbg/$(basename $f .cu).o &
 done
 wait
-nvcc -shared -o tools/build/librmd_b200_dbg.so tools/build/dbg/*.o -gencode arch=compute_90a,code=sm_90a -lpthread
+nvcc -shared -o tools/build/librmd_b200_dbg.so tools/build/dbg/*.o -gencode arch=compute_90a,code=sm_90a -lpthread -ldl
 ls -la tools/build/librmd_b200_dbg.so

@@ -8,6 +8,7 @@ import rpg_open_remode_b200 as rmd
 from rpg_open_remode_b200 import synth
 
 W, H, N = (int(v) for v in os.environ.get('RMD_PROBE_SIZE', '640,480,200').split(','))
+RUN = int(os.environ['RMD_PROBE_RUN']) if 'RMD_PROBE_RUN' in os.environ else None   # OPT_TUNE_RUN_CHUNKS (unset: the default)
 seq = synth.SyntheticSequence(W, H, seed=0x5EED0002)
 frames = np.empty((N, H, W), np.float32); poses = np.empty((N, 12), np.float32)
 for k in range(N):
@@ -26,6 +27,7 @@ def full(cfg):
 def run(cfg):
     cfg = full(cfg)
     for opt, val in zip((10, 11, 12, 13, 14, 15, 16, 17, 5, 6, 18, 19, 20), cfg): g.setOption(opt, val)
+    if RUN is not None: g.setOption(rmd.OPT_TUNE_RUN_CHUNKS, RUN)
     best = 1e9; seg = None
     for rep in range(4):
         g.setReferenceImageDevice(d_frames[0].data_ptr(), W * 4, poses[0], dmin, dmax)
@@ -48,5 +50,5 @@ if len(sys.argv) > 1:
     CONFIGS = [tuple(int(v) for v in a.split(",")) for a in sys.argv[1:]]
 for cfg in CONFIGS:
     tot, seg = run(cfg)
-    print("split_max %2d min_items %4d per_cta %4d sparse %3d heavy_min %5d avg_pct %3d pdl %d warp_tiles %d chain %d seed_pct %d grid %d ctas/sm %d wt_cands %d : total %.2f ms (%.0f fps)  frames1-19 %.2f  20-99 %.2f  100-end %.2f ms" %
-          (*(tuple(cfg) + (0,) * (12 - len(cfg)) if len(cfg) < 13 else tuple(cfg)), tot, (N - 1) / tot * 1e3, *seg), flush=True)
+    print(("run %d " % RUN if RUN is not None else "") + "split_max %2d min_items %4d per_cta %4d sparse %3d heavy_min %5d avg_pct %3d pdl %d warp_tiles %d chain %d seed_pct %d grid %d ctas/sm %d wt_cands %d : total %.2f ms (%.0f fps)  frames1-19 %.2f  20-99 %.2f  100-end %.2f ms" %
+          (*full(cfg), tot, (N - 1) / tot * 1e3, *seg), flush=True)
