@@ -15,7 +15,7 @@ _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "librmd_b200.so")
 
 CUDA_SOURCES = ["c_api.cu", "depth_filter.cu", "depth_filter_staged.cu", "depth_filter_seeds.cu", "denoiser.cu", "reduction.cu", "ingest.cu", "point_cloud.cu",
-                "prior.cu", "volume.cu", "multi_gpu.cu"]
+                "prior.cu", "volume.cu", "volume_api.cu", "multi_gpu.cu"]
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3",

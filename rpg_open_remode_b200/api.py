@@ -580,30 +580,26 @@ class TsdfVolume:
         if keep:
             self.sync()   # the staged images must outlive the kernel
 
+    def _surface(self, fn, capacity, shape, what: str) -> np.ndarray:
+        """One float32 [shape] per surface point from fn (rmd_volume_surface_points or _intensity): the count first
+        when no capacity is given, then at most capacity of them."""
+        n = ctypes.c_size_t()
+        if capacity is None:
+            check(fn(self._h, None, 0, ctypes.byref(n)), what)
+            capacity = n.value
+        out = np.empty((int(capacity),) + shape, np.float32)
+        check(fn(self._h, out.ctypes.data if capacity else None, int(capacity), ctypes.byref(n)), what)
+        return out[:min(int(capacity), n.value)]
+
     def surfacePoints(self, capacity: "int | None" = None) -> np.ndarray:
         """float32 [n, 4] = (x, y, z, weight) of the zero crossings, in voxel order then axis x, y, z.  With a
         capacity, at most that many points."""
-        n = ctypes.c_size_t()
-        if capacity is None:
-            check(self._L.rmd_volume_surface_points(self._h, None, 0, ctypes.byref(n)), "TsdfVolume::surfacePoints")
-            capacity = n.value
-        out = np.empty((int(capacity), 4), np.float32)
-        check(self._L.rmd_volume_surface_points(self._h, out.ctypes.data if capacity else None, int(capacity),
-                                                ctypes.byref(n)), "TsdfVolume::surfacePoints")
-        return out[:min(int(capacity), n.value)]
+        return self._surface(self._L.rmd_volume_surface_points, capacity, (4,), "TsdfVolume::surfacePoints")
 
     def surfaceIntensity(self, capacity: "int | None" = None) -> np.ndarray:
         """float32 [n]: the intensity of every surface point (and mesh vertex), in surfacePoints() order; -1 where
         neither of the point's voxels has one.  With a capacity, at most that many."""
-        n = ctypes.c_size_t()
-        if capacity is None:
-            check(self._L.rmd_volume_surface_intensity(self._h, None, 0, ctypes.byref(n)),
-                  "TsdfVolume::surfaceIntensity")
-            capacity = n.value
-        out = np.empty(int(capacity), np.float32)
-        check(self._L.rmd_volume_surface_intensity(self._h, out.ctypes.data if capacity else None, int(capacity),
-                                                   ctypes.byref(n)), "TsdfVolume::surfaceIntensity")
-        return out[:min(int(capacity), n.value)]
+        return self._surface(self._L.rmd_volume_surface_intensity, capacity, (), "TsdfVolume::surfaceIntensity")
 
     def mesh(self, vertex_capacity: "int | None" = None, triangle_capacity: "int | None" = None):
         """Marching-cubes mesh of the fused surface: (float32 [n, 4] vertices, int32 [m, 3] triangles).  The vertices
@@ -643,35 +639,33 @@ class TsdfVolume:
         self.sync()
         return img.getDevData(), inten.getDevData()
 
+    def _download_records(self, fn, what: str):
+        """The two halves of a record array (fn: rmd_volume_download[_intensity]), float32 of shape (nz, ny, nx)."""
+        nx, ny, nz = self.dims
+        a, b = np.empty((nz, ny, nx), np.float32), np.empty((nz, ny, nx), np.float32)
+        check(fn(self._h, a.ctypes.data, b.ctypes.data), what)
+        return a, b
+
+    def _upload_records(self, fn, a, b, what: str) -> None:
+        nx, ny, nz = self.dims
+        a, b = (np.ascontiguousarray(x, np.float32) for x in (a, b))
+        if a.size != nx * ny * nz or b.size != nx * ny * nz:
+            raise ValueError(what + ": wrong size")
+        check(fn(self._h, a.ctypes.data, b.ctypes.data), what)
+
     def download(self):
         """(tsdf, weight), float32 arrays of shape (nz, ny, nx)."""
-        nx, ny, nz = self.dims
-        t, w = np.empty((nz, ny, nx), np.float32), np.empty((nz, ny, nx), np.float32)
-        check(self._L.rmd_volume_download(self._h, t.ctypes.data, w.ctypes.data), "TsdfVolume::download")
-        return t, w
+        return self._download_records(self._L.rmd_volume_download, "TsdfVolume::download")
 
     def upload(self, tsdf, weight) -> None:
-        nx, ny, nz = self.dims
-        t, w = (np.ascontiguousarray(a, np.float32) for a in (tsdf, weight))
-        if t.size != nx * ny * nz or w.size != nx * ny * nz:
-            raise ValueError("TsdfVolume::upload: wrong size")
-        check(self._L.rmd_volume_upload(self._h, t.ctypes.data, w.ctypes.data), "TsdfVolume::upload")
+        self._upload_records(self._L.rmd_volume_upload, tsdf, weight, "TsdfVolume::upload")
 
     def downloadIntensity(self):
         """(intensity, intensity weight), float32 arrays of shape (nz, ny, nx)."""
-        nx, ny, nz = self.dims
-        c, w = np.empty((nz, ny, nx), np.float32), np.empty((nz, ny, nx), np.float32)
-        check(self._L.rmd_volume_download_intensity(self._h, c.ctypes.data, w.ctypes.data),
-              "TsdfVolume::downloadIntensity")
-        return c, w
+        return self._download_records(self._L.rmd_volume_download_intensity, "TsdfVolume::downloadIntensity")
 
     def uploadIntensity(self, intensity, weight) -> None:
-        nx, ny, nz = self.dims
-        c, w = (np.ascontiguousarray(a, np.float32) for a in (intensity, weight))
-        if c.size != nx * ny * nz or w.size != nx * ny * nz:
-            raise ValueError("TsdfVolume::uploadIntensity: wrong size")
-        check(self._L.rmd_volume_upload_intensity(self._h, c.ctypes.data, w.ctypes.data),
-              "TsdfVolume::uploadIntensity")
+        self._upload_records(self._L.rmd_volume_upload_intensity, intensity, weight, "TsdfVolume::uploadIntensity")
 
     def reset(self) -> None:
         check(self._L.rmd_volume_reset(self._h), "TsdfVolume::reset")

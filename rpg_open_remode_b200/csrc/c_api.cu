@@ -6,7 +6,8 @@
 // (include/rmd/device_image.cuh), re-designed: per-handle streams instead of
 // the legacy default stream, a pinned upload ring with a copy stream so the
 // H2D transfer of frame k+1 overlaps the kernel of frame k, one fused launch
-// per frame and no device synchronisation inside update().
+// per frame and no device synchronisation inside update().  The TSDF volume's entry points are in volume_api.cu,
+// except rmd_volume_integrate_seeds, which reads the seeds' internals.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -2097,293 +2098,11 @@ int rmd_image_copy(void *dst, size_t dst_pitch, const void *src, size_t src_pitc
 } // extern "C"
 
 // ============================================================ TSDF volume
-
-struct rmd_volume
-{
-  int device;
-  VolumeGrid g;               // g.vox: nx * ny * nz float2 (tsdf, weight)
-  size_t n_vox;
-  float trunc, max_weight;
-  cudaStream_t own_stream, stream;
-  cudaEvent_t seeds_ev;       // integrate_seeds: the seeds' stream has produced what the kernel reads
-  // surface points (allocated on first use): per-block offsets, total, host staging grown on demand
-  unsigned long long *surf_offsets, *surf_total;
-  float4 *stage; size_t stage_cap;
-  // mesh (allocated on first use): per-block triangle offsets and total, the points' keys and the host variant's
-  // triangle staging, grown on demand
-  unsigned long long *tri_offsets, *tri_total;
-  unsigned long long *keys; size_t keys_cap;
-  int *tri_stage; size_t tri_stage_cap;
-  // intensity channel (rmd_volume_enable_intensity; NULL = off): n_vox float2 (intensity, weight), indexed like
-  // g.vox, and the host variant's staging of the surface intensities, grown on demand
-  float2 *col;
-  float *istage; size_t istage_cap;
-  uint64_t n_total;
-};
-
-namespace
-{
-
-const size_t kVolumeMaxVoxels = (size_t)1 << 31;
-const size_t kVolumeChunk = (size_t)1 << 24;   // voxels per host staging chunk of download / upload
-
-bool depth_pitch_ok(size_t pitch, int width)
-{
-  return pitch >= sizeof(float) * (size_t)width && pitch % sizeof(float) == 0;
-}
-
-// intensity (NULL = the tsdf only): an image of the depth's size, fused into v->col
-int volume_integrate(rmd_volume *v, int width, int height, const Camera &cam, const Pose &T_curr_world,
-                     const float *depth, size_t depth_stride, int depth_comps, const int32_t *conv, size_t conv_stride,
-                     const float *intensity = NULL, size_t intensity_stride = 0)
-{
-  VolumeIntegrateParams P;
-  memset(&P, 0, sizeof(P));
-  P.g = v->g;
-  P.width = width; P.height = height;
-  P.cam = cam;
-  P.T_curr_world = T_curr_world;
-  P.depth = depth; P.depth_stride = depth_stride; P.depth_comps = depth_comps;
-  P.conv = conv; P.conv_stride = conv_stride;
-  P.trunc = v->trunc; P.max_weight = v->max_weight;
-  if(intensity)
-  {
-    P.col = v->col;
-    P.intensity = intensity; P.intensity_stride = intensity_stride;
-  }
-  RMD_CUDA_TRY(launch_volume_integrate(P, v->stream));
-  v->n_total += 1;
-  return 0;
-}
-
-// Count pass + scan: returns the number of surface points (synchronises the volume's stream).
-int volume_surface_count(rmd_volume *v, VolumeSurfaceParams &P, size_t *count)
-{
-  memset(&P, 0, sizeof(P));
-  P.g = v->g;
-  P.n_blocks = (unsigned int)((v->n_vox + VOLUME_SURF_VOXELS - 1) / VOLUME_SURF_VOXELS);
-  if(!v->surf_offsets)
-  {
-    RMD_CUDA_TRY(cudaMalloc(&v->surf_offsets, sizeof(unsigned long long) * P.n_blocks));
-    RMD_CUDA_TRY(cudaMalloc(&v->surf_total, sizeof(unsigned long long)));
-  }
-  P.block_offsets = v->surf_offsets;
-  P.total = v->surf_total;
-  RMD_CUDA_TRY(launch_volume_surface_count(P, v->stream));
-  v->n_total += 2;
-  unsigned long long n = 0;
-  RMD_CUDA_TRY(cudaMemcpyAsync(&n, v->surf_total, sizeof(n), cudaMemcpyDeviceToHost, v->stream));
-  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
-  *count = (size_t)n;
-  return 0;
-}
-
-int volume_surface_write(rmd_volume *v, VolumeSurfaceParams &P, float4 *out, size_t capacity)
-{
-  P.out = out;
-  P.capacity = capacity;
-  RMD_CUDA_TRY(launch_volume_surface_write(P, v->stream));
-  v->n_total += 1;
-  return 0;
-}
-
-// Device buffer of at least n elements, grown (never shrunk) on demand.
-template<typename T>
-int volume_grow(T **buf, size_t *cap, size_t n)
-{
-  if(n <= *cap)
-    return 0;
-  RMD_CUDA_TRY(cudaFree(*buf));
-  *buf = NULL; *cap = 0;
-  RMD_CUDA_TRY(cudaMalloc(buf, sizeof(T) * n));
-  *cap = n;
-  return 0;
-}
-
-// The mesh: both count passes and scans, one host read of the two totals, then -- for what the capacities ask --
-// the surface points (with their keys when triangles are wanted) and the triangles.  host: min(count, capacity)
-// of each are staged in the volume's buffers and copied to xyzw / tri.  Synchronous.
-int volume_mesh(rmd_volume *v, void *xyzw, size_t vertex_capacity, int32_t *tri, size_t tri_capacity,
-                size_t *n_vertices, size_t *n_triangles, bool host, const char *what)
-{
-  VolumeSurfaceParams S;
-  memset(&S, 0, sizeof(S));
-  S.g = v->g;
-  S.n_blocks = (unsigned int)((v->n_vox + VOLUME_SURF_VOXELS - 1) / VOLUME_SURF_VOXELS);
-  if(!v->surf_offsets)
-  {
-    RMD_CUDA_TRY(cudaMalloc(&v->surf_offsets, sizeof(unsigned long long) * S.n_blocks));
-    RMD_CUDA_TRY(cudaMalloc(&v->surf_total, sizeof(unsigned long long)));
-  }
-  if(!v->tri_offsets)
-  {
-    RMD_CUDA_TRY(cudaMalloc(&v->tri_offsets, sizeof(unsigned long long) * S.n_blocks));
-    RMD_CUDA_TRY(cudaMalloc(&v->tri_total, sizeof(unsigned long long)));
-  }
-  S.block_offsets = v->surf_offsets;
-  S.total = v->surf_total;
-  VolumeMeshParams M;
-  memset(&M, 0, sizeof(M));
-  M.g = v->g;
-  M.point_offsets = v->surf_offsets;
-  M.point_total = v->surf_total;
-  M.block_offsets = v->tri_offsets;
-  M.total = v->tri_total;
-  M.n_blocks = S.n_blocks;
-  RMD_CUDA_TRY(launch_volume_surface_count(S, v->stream));
-  RMD_CUDA_TRY(launch_volume_mesh_count(M, v->stream));
-  v->n_total += 4;
-  unsigned long long nv = 0, nt = 0;
-  RMD_CUDA_TRY(cudaMemcpyAsync(&nv, v->surf_total, sizeof(nv), cudaMemcpyDeviceToHost, v->stream));
-  RMD_CUDA_TRY(cudaMemcpyAsync(&nt, v->tri_total, sizeof(nt), cudaMemcpyDeviceToHost, v->stream));
-  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
-  *n_vertices = (size_t)nv;
-  *n_triangles = (size_t)nt;
-  if(nv >= (1ull << 31))
-    return fail(RMD_ERR_UNSUPPORTED, (std::string(what) + ": 2^31 or more vertices do not fit int32 indices").c_str());
-  const size_t mv = nv < vertex_capacity ? (size_t)nv : vertex_capacity;
-  const size_t mt = nt < tri_capacity ? (size_t)nt : tri_capacity;
-  if(!mv && !mt)
-    return 0;
-  float4 *vout = reinterpret_cast<float4*>(xyzw);
-  int *tout = tri;
-  if(host)
-  {
-    int rc = volume_grow(&v->stage, &v->stage_cap, mv);
-    if(!rc) rc = volume_grow(&v->tri_stage, &v->tri_stage_cap, 3 * mt);
-    if(rc) return rc;
-    vout = v->stage;
-    tout = v->tri_stage;
-  }
-  S.out = vout;
-  S.capacity = mv;
-  if(mt)
-  {
-    // every vertex's key, whatever the vertex capacity: triangles may index vertices that are not returned
-    const int rc = volume_grow(&v->keys, &v->keys_cap, (size_t)nv);
-    if(rc) return rc;
-    S.keys = v->keys;
-    RMD_CUDA_TRY(launch_volume_surface_write_keys(S, v->stream));
-    M.keys = v->keys;
-    M.tri = tout;
-    M.capacity = mt;
-    RMD_CUDA_TRY(launch_volume_mesh_write(M, v->stream));
-    v->n_total += 2;
-  }
-  else
-  {
-    RMD_CUDA_TRY(launch_volume_surface_write(S, v->stream));
-    v->n_total += 1;
-  }
-  if(host)
-  {
-    if(mv)
-      RMD_CUDA_TRY(cudaMemcpyAsync(xyzw, v->stage, mv * sizeof(float4), cudaMemcpyDeviceToHost, v->stream));
-    if(mt)
-      RMD_CUDA_TRY(cudaMemcpyAsync(tri, v->tri_stage, mt * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, v->stream));
-  }
-  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
-  return 0;
-}
-
-} // namespace
+// The volume's entry points are in volume_api.cu; this one reads the seeds' internals and orders the volume's
+// stream against theirs.
 
 extern "C"
 {
-
-int rmd_volume_create(int nx, int ny, int nz, float voxel_size, const float origin[3], float truncation,
-                      float max_weight, int device, rmd_volume_t **out)
-{
-  RMD_REQUIRE(out, "rmd_volume_create: out is null");
-  *out = NULL;
-  RMD_REQUIRE(origin, "rmd_volume_create: origin is null");
-  RMD_REQUIRE(nx > 0 && ny > 0 && nz > 0, "rmd_volume_create: grid dimensions must be positive");
-  const uint64_t plane = (uint64_t)nx * (uint64_t)ny;   // each factor < 2^31: no overflow in 64 bits
-  RMD_REQUIRE(plane <= kVolumeMaxVoxels && plane * (uint64_t)nz <= kVolumeMaxVoxels,
-              "rmd_volume_create: at most 2^31 voxels");
-  RMD_REQUIRE(voxel_size > 0.0f && isfinite(voxel_size), "rmd_volume_create: voxel_size must be > 0");
-  RMD_REQUIRE(truncation > 0.0f && isfinite(truncation), "rmd_volume_create: truncation must be > 0");
-  RMD_REQUIRE(max_weight >= 1.0f, "rmd_volume_create: max_weight must be >= 1");
-  RMD_REQUIRE(isfinite(origin[0]) && isfinite(origin[1]) && isfinite(origin[2]), "rmd_volume_create: bad origin");
-  if(device < 0) RMD_CUDA_TRY(cudaGetDevice(&device));
-  DeviceGuard guard(device);
-  rmd_volume *v = new(std::nothrow) rmd_volume();
-  if(!v) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_create: host allocation failed");
-  memset(v, 0, sizeof(*v));
-  v->device = device;
-  v->g.nx = nx; v->g.ny = ny; v->g.nz = nz;
-  v->g.voxel = voxel_size;
-  v->g.ox = origin[0]; v->g.oy = origin[1]; v->g.oz = origin[2];
-  v->n_vox = (size_t)(plane * (uint64_t)nz);
-  v->trunc = truncation; v->max_weight = max_weight;
-  cudaError_t err = cudaStreamCreateWithFlags(&v->own_stream, cudaStreamNonBlocking);
-  if(err == cudaSuccess) err = cudaEventCreateWithFlags(&v->seeds_ev, cudaEventDisableTiming);
-  if(err == cudaSuccess) err = cudaMalloc(&v->g.vox, sizeof(float2) * v->n_vox);
-  if(err == cudaSuccess) err = cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->own_stream);
-  if(err == cudaSuccess) err = cudaStreamSynchronize(v->own_stream);
-  if(err != cudaSuccess)
-  {
-    rmd_volume_destroy(v);
-    return fail_cuda(err, "rmd_volume_create");
-  }
-  v->stream = v->own_stream;
-  *out = v;
-  return 0;
-}
-
-int rmd_volume_destroy(rmd_volume_t *v)
-{
-  if(!v) return 0;
-  DeviceGuard guard(v->device);
-  cudaDeviceSynchronize();
-  if(v->own_stream) cudaStreamDestroy(v->own_stream);
-  if(v->seeds_ev) cudaEventDestroy(v->seeds_ev);
-  cudaFree(v->g.vox);
-  cudaFree(v->surf_offsets); cudaFree(v->surf_total); cudaFree(v->stage);
-  cudaFree(v->tri_offsets); cudaFree(v->tri_total); cudaFree(v->keys); cudaFree(v->tri_stage);
-  cudaFree(v->col); cudaFree(v->istage);
-  cudaGetLastError();
-  delete v;
-  return 0;
-}
-
-int rmd_volume_set_stream(rmd_volume_t *v, void *cuda_stream)
-{
-  RMD_REQUIRE(v, "rmd_volume_set_stream: null handle");
-  DeviceGuard guard(v->device);
-  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
-  v->stream = cuda_stream ? (cudaStream_t)cuda_stream : v->own_stream;
-  return 0;
-}
-
-int rmd_volume_reset(rmd_volume_t *v)
-{
-  RMD_REQUIRE(v, "rmd_volume_reset: null handle");
-  DeviceGuard guard(v->device);
-  RMD_CUDA_TRY(cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->stream));
-  if(v->col)
-    RMD_CUDA_TRY(cudaMemsetAsync(v->col, 0, sizeof(float2) * v->n_vox, v->stream));
-  return 0;
-}
-
-int rmd_volume_sync(rmd_volume_t *v)
-{
-  RMD_REQUIRE(v, "rmd_volume_sync: null handle");
-  DeviceGuard guard(v->device);
-  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
-  return 0;
-}
-
-int rmd_volume_size(rmd_volume_t *v, int *nx, int *ny, int *nz, float *voxel_size, float origin[3])
-{
-  RMD_REQUIRE(v, "rmd_volume_size: null handle");
-  if(nx) *nx = v->g.nx;
-  if(ny) *ny = v->g.ny;
-  if(nz) *nz = v->g.nz;
-  if(voxel_size) *voxel_size = v->g.voxel;
-  if(origin) { origin[0] = v->g.ox; origin[1] = v->g.oy; origin[2] = v->g.oz; }
-  return 0;
-}
 
 int rmd_volume_integrate_seeds(rmd_volume_t *v, rmd_seeds_t *s, const float *dev_depth, size_t depth_pitch)
 {
@@ -2399,349 +2118,29 @@ int rmd_volume_integrate_seeds(rmd_volume_t *v, rmd_seeds_t *s, const float *dev
   RMD_CUDA_TRY(cudaStreamWaitEvent(v->stream, v->seeds_ev, 0));
   if(s->ext_pending)
     RMD_CUDA_TRY(cudaStreamWaitEvent(v->stream, s->ext_ev, 0));
-  // with the intensity channel, the reference image is fused too
-  const float *ref = v->col ? s->ref : NULL;
-  const size_t ref_stride = s->ref_pitch / sizeof(float);
-  const int rc = dev_depth
-      ? volume_integrate(v, s->width, s->height, s->cam, s->T_ref_world, dev_depth, depth_pitch / sizeof(float), 1,
-                         s->conv, s->conv_pitch / sizeof(int), ref, ref_stride)
-      : volume_integrate(v, s->width, s->height, s->cam, s->T_ref_world, reinterpret_cast<const float*>(s->seed),
-                         (size_t)s->seed_stride * 4, 4, s->conv, s->conv_pitch / sizeof(int), ref, ref_stride);
+  VolumeIntegrateParams P;
+  memset(&P, 0, sizeof(P));
+  P.width = s->width; P.height = s->height;
+  P.cam = s->cam;
+  P.T_curr_world = s->T_ref_world;
+  if(dev_depth)
+  {
+    P.depth = dev_depth; P.depth_stride = depth_pitch / sizeof(float); P.depth_comps = 1;
+  }
+  else
+  {
+    P.depth = reinterpret_cast<const float*>(s->seed); P.depth_stride = (size_t)s->seed_stride * 4; P.depth_comps = 4;
+  }
+  P.conv = s->conv; P.conv_stride = s->conv_pitch / sizeof(int);
+  if(v->col)   // with the intensity channel, the reference image is fused too
+  {
+    P.intensity = s->ref; P.intensity_stride = s->ref_pitch / sizeof(float);
+  }
+  const int rc = volume_integrate(v, P);
   if(rc) return rc;
   // ... and a later writer of the seeds (update, set_reference, upload_state) waits for the kernel's reads
   RMD_CUDA_TRY(cudaEventRecord(s->ext_ev, v->stream));
   s->ext_pending = true;
-  return 0;
-}
-
-int rmd_volume_integrate_depth(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
-                               const float *T_curr_world, const float *dev_depth, size_t depth_pitch,
-                               const int32_t *dev_conv, size_t conv_pitch)
-{
-  RMD_REQUIRE(v && T_curr_world && dev_depth, "rmd_volume_integrate_depth: null argument");
-  RMD_REQUIRE(width > 0 && height > 0, "rmd_volume_integrate_depth: bad image size");
-  RMD_REQUIRE(depth_pitch_ok(depth_pitch, width), "rmd_volume_integrate_depth: bad depth pitch");
-  RMD_REQUIRE(!dev_conv || (conv_pitch >= sizeof(int32_t) * (size_t)width && conv_pitch % sizeof(int32_t) == 0),
-              "rmd_volume_integrate_depth: bad state pitch");
-  DeviceGuard guard(v->device);
-  Camera cam;
-  cam.fx = fx; cam.fy = fy; cam.cx = cx; cam.cy = cy;
-  return volume_integrate(v, width, height, cam, pose_from(T_curr_world), dev_depth, depth_pitch / sizeof(float), 1,
-                          dev_conv, conv_pitch / sizeof(int32_t));
-}
-
-int rmd_volume_surface_points(rmd_volume_t *v, float *host_xyzw, size_t capacity, size_t *count)
-{
-  RMD_REQUIRE(v && count && (host_xyzw || capacity == 0), "rmd_volume_surface_points: null argument");
-  DeviceGuard guard(v->device);
-  VolumeSurfaceParams P;
-  {
-    const int rc = volume_surface_count(v, P, count);
-    if(rc) return rc;
-  }
-  const size_t n = *count < capacity ? *count : capacity;
-  if(!n)
-    return 0;
-  if(n > v->stage_cap)
-  {
-    RMD_CUDA_TRY(cudaFree(v->stage));
-    v->stage = NULL; v->stage_cap = 0;
-    RMD_CUDA_TRY(cudaMalloc(&v->stage, sizeof(float4) * n));
-    v->stage_cap = n;
-  }
-  {
-    const int rc = volume_surface_write(v, P, v->stage, n);
-    if(rc) return rc;
-  }
-  RMD_CUDA_TRY(cudaMemcpyAsync(host_xyzw, v->stage, n * sizeof(float4), cudaMemcpyDeviceToHost, v->stream));
-  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
-  return 0;
-}
-
-int rmd_volume_surface_points_device(rmd_volume_t *v, float *dev_xyzw, size_t capacity, size_t *count)
-{
-  RMD_REQUIRE(v && count && (dev_xyzw || capacity == 0), "rmd_volume_surface_points_device: null argument");
-  RMD_REQUIRE(((uintptr_t)dev_xyzw % 16) == 0, "rmd_volume_surface_points_device: output must be 16-byte aligned");
-  DeviceGuard guard(v->device);
-  VolumeSurfaceParams P;
-  {
-    const int rc = volume_surface_count(v, P, count);
-    if(rc) return rc;
-  }
-  const size_t n = *count < capacity ? *count : capacity;
-  if(!n)
-    return 0;
-  {
-    const int rc = volume_surface_write(v, P, reinterpret_cast<float4*>(dev_xyzw), n);
-    if(rc) return rc;
-  }
-  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
-  return 0;
-}
-
-int rmd_volume_mesh(rmd_volume_t *v, float *host_xyzw, size_t vertex_capacity, int32_t *host_tri,
-                    size_t tri_capacity, size_t *n_vertices, size_t *n_triangles)
-{
-  RMD_REQUIRE(v && n_vertices && n_triangles && (host_xyzw || vertex_capacity == 0) && (host_tri || tri_capacity == 0),
-              "rmd_volume_mesh: null argument");
-  DeviceGuard guard(v->device);
-  return volume_mesh(v, host_xyzw, vertex_capacity, host_tri, tri_capacity, n_vertices, n_triangles, true,
-                     "rmd_volume_mesh");
-}
-
-int rmd_volume_mesh_device(rmd_volume_t *v, float *dev_xyzw, size_t vertex_capacity, int32_t *dev_tri,
-                           size_t tri_capacity, size_t *n_vertices, size_t *n_triangles)
-{
-  RMD_REQUIRE(v && n_vertices && n_triangles && (dev_xyzw || vertex_capacity == 0) && (dev_tri || tri_capacity == 0),
-              "rmd_volume_mesh_device: null argument");
-  RMD_REQUIRE(((uintptr_t)dev_xyzw % 16) == 0, "rmd_volume_mesh_device: vertices must be 16-byte aligned");
-  RMD_REQUIRE(((uintptr_t)dev_tri % 4) == 0, "rmd_volume_mesh_device: triangles must be 4-byte aligned");
-  DeviceGuard guard(v->device);
-  return volume_mesh(v, dev_xyzw, vertex_capacity, dev_tri, tri_capacity, n_vertices, n_triangles, false,
-                     "rmd_volume_mesh_device");
-}
-
-int rmd_volume_raycast(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
-                       const float *T_curr_world, float *dev_depth, size_t depth_pitch)
-{
-  RMD_REQUIRE(v && T_curr_world && dev_depth, "rmd_volume_raycast: null argument");
-  RMD_REQUIRE(width > 0 && height > 0, "rmd_volume_raycast: bad image size");
-  RMD_REQUIRE(depth_pitch_ok(depth_pitch, width), "rmd_volume_raycast: bad depth pitch");
-  DeviceGuard guard(v->device);
-  VolumeRaycastParams P;
-  memset(&P, 0, sizeof(P));
-  P.g = v->g;
-  P.width = width; P.height = height;
-  P.cam.fx = fx; P.cam.fy = fy; P.cam.cx = cx; P.cam.cy = cy;
-  P.T_world_curr = pose_inverse(pose_from(T_curr_world));
-  P.depth = dev_depth; P.depth_stride = depth_pitch / sizeof(float);
-  RMD_CUDA_TRY(launch_volume_raycast(P, v->stream));
-  v->n_total += 1;
-  return 0;
-}
-
-int rmd_volume_download(rmd_volume_t *v, float *host_tsdf, float *host_weight)
-{
-  RMD_REQUIRE(v && host_tsdf && host_weight, "rmd_volume_download: null argument");
-  DeviceGuard guard(v->device);
-  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
-  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
-  if(!tmp) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_download: host allocation failed");
-  cudaError_t err = cudaSuccess;
-  for(size_t b = 0; b < v->n_vox && err == cudaSuccess; b += chunk)
-  {
-    const size_t m = v->n_vox - b < chunk ? v->n_vox - b : chunk;
-    err = cudaMemcpyAsync(tmp, v->g.vox + b, sizeof(float2) * m, cudaMemcpyDeviceToHost, v->stream);
-    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);
-    for(size_t q = 0; q < m && err == cudaSuccess; ++q)
-    {
-      host_tsdf[b + q] = tmp[q].x;
-      host_weight[b + q] = tmp[q].y;
-    }
-  }
-  free(tmp);
-  RMD_CUDA_TRY(err);
-  return 0;
-}
-
-int rmd_volume_upload(rmd_volume_t *v, const float *host_tsdf, const float *host_weight)
-{
-  RMD_REQUIRE(v && host_tsdf && host_weight, "rmd_volume_upload: null argument");
-  DeviceGuard guard(v->device);
-  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
-  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
-  if(!tmp) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_upload: host allocation failed");
-  cudaError_t err = cudaSuccess;
-  for(size_t b = 0; b < v->n_vox && err == cudaSuccess; b += chunk)
-  {
-    const size_t m = v->n_vox - b < chunk ? v->n_vox - b : chunk;
-    for(size_t q = 0; q < m; ++q)
-      tmp[q] = make_float2(host_tsdf[b + q], host_weight[b + q]);
-    err = cudaMemcpyAsync(v->g.vox + b, tmp, sizeof(float2) * m, cudaMemcpyHostToDevice, v->stream);
-    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);   // tmp is refilled next
-  }
-  free(tmp);
-  RMD_CUDA_TRY(err);
-  return 0;
-}
-
-} // extern "C"
-
-// ============================================================ TSDF volume: intensity channel
-
-namespace
-{
-
-// Surface intensities: the surface points' count pass and scan, then their write pass in its intensity instance
-// (same blocks, same ranks).  host: min(count, capacity) are staged in v->istage and copied to out.  Synchronous.
-int volume_surface_intensity(rmd_volume *v, float *out, size_t capacity, size_t *count, bool host)
-{
-  VolumeSurfaceParams P;
-  {
-    const int rc = volume_surface_count(v, P, count);
-    if(rc) return rc;
-  }
-  const size_t n = *count < capacity ? *count : capacity;
-  if(!n)
-    return 0;
-  if(host)
-  {
-    const int rc = volume_grow(&v->istage, &v->istage_cap, n);
-    if(rc) return rc;
-  }
-  P.col = v->col;
-  P.intensity = host ? v->istage : out;
-  P.capacity = n;
-  RMD_CUDA_TRY(launch_volume_surface_write_intensity(P, v->stream));
-  v->n_total += 1;
-  if(host)
-    RMD_CUDA_TRY(cudaMemcpyAsync(out, v->istage, n * sizeof(float), cudaMemcpyDeviceToHost, v->stream));
-  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
-  return 0;
-}
-
-int no_intensity(const char *what)
-{
-  return fail(RMD_ERR_NOT_INITIALISED, (std::string(what) + ": the volume has no intensity channel").c_str());
-}
-
-} // namespace
-
-extern "C"
-{
-
-int rmd_volume_enable_intensity(rmd_volume_t *v)
-{
-  RMD_REQUIRE(v, "rmd_volume_enable_intensity: null handle");
-  if(v->col)
-    return 0;
-  DeviceGuard guard(v->device);
-  cudaError_t err = cudaMalloc(&v->col, sizeof(float2) * v->n_vox);
-  if(err != cudaSuccess)
-  {
-    v->col = NULL;
-    return fail_cuda(err, "rmd_volume_enable_intensity");
-  }
-  err = cudaMemsetAsync(v->col, 0, sizeof(float2) * v->n_vox, v->stream);
-  if(err != cudaSuccess)
-  {
-    cudaFree(v->col);
-    v->col = NULL;
-    return fail_cuda(err, "rmd_volume_enable_intensity");
-  }
-  return 0;
-}
-
-int rmd_volume_integrate_depth_intensity(rmd_volume_t *v, int width, int height, float fx, float fy, float cx,
-                                         float cy, const float *T_curr_world, const float *dev_depth,
-                                         size_t depth_pitch, const int32_t *dev_conv, size_t conv_pitch,
-                                         const float *dev_intensity, size_t intensity_pitch)
-{
-  RMD_REQUIRE(v && T_curr_world && dev_depth && dev_intensity, "rmd_volume_integrate_depth_intensity: null argument");
-  RMD_REQUIRE(width > 0 && height > 0, "rmd_volume_integrate_depth_intensity: bad image size");
-  RMD_REQUIRE(depth_pitch_ok(depth_pitch, width), "rmd_volume_integrate_depth_intensity: bad depth pitch");
-  RMD_REQUIRE(!dev_conv || (conv_pitch >= sizeof(int32_t) * (size_t)width && conv_pitch % sizeof(int32_t) == 0),
-              "rmd_volume_integrate_depth_intensity: bad state pitch");
-  RMD_REQUIRE(depth_pitch_ok(intensity_pitch, width), "rmd_volume_integrate_depth_intensity: bad intensity pitch");
-  if(!v->col)
-    return no_intensity("rmd_volume_integrate_depth_intensity");
-  DeviceGuard guard(v->device);
-  Camera cam;
-  cam.fx = fx; cam.fy = fy; cam.cx = cx; cam.cy = cy;
-  return volume_integrate(v, width, height, cam, pose_from(T_curr_world), dev_depth, depth_pitch / sizeof(float), 1,
-                          dev_conv, conv_pitch / sizeof(int32_t), dev_intensity, intensity_pitch / sizeof(float));
-}
-
-int rmd_volume_surface_intensity(rmd_volume_t *v, float *host_intensity, size_t capacity, size_t *count)
-{
-  RMD_REQUIRE(v && count && (host_intensity || capacity == 0), "rmd_volume_surface_intensity: null argument");
-  if(!v->col)
-    return no_intensity("rmd_volume_surface_intensity");
-  DeviceGuard guard(v->device);
-  return volume_surface_intensity(v, host_intensity, capacity, count, true);
-}
-
-int rmd_volume_surface_intensity_device(rmd_volume_t *v, float *dev_intensity, size_t capacity, size_t *count)
-{
-  RMD_REQUIRE(v && count && (dev_intensity || capacity == 0), "rmd_volume_surface_intensity_device: null argument");
-  RMD_REQUIRE(((uintptr_t)dev_intensity % 4) == 0, "rmd_volume_surface_intensity_device: output must be 4-byte aligned");
-  if(!v->col)
-    return no_intensity("rmd_volume_surface_intensity_device");
-  DeviceGuard guard(v->device);
-  return volume_surface_intensity(v, dev_intensity, capacity, count, false);
-}
-
-int rmd_volume_raycast_intensity(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
-                                 const float *T_curr_world, float *dev_depth, size_t depth_pitch,
-                                 float *dev_intensity, size_t intensity_pitch)
-{
-  RMD_REQUIRE(v && T_curr_world && dev_depth && dev_intensity, "rmd_volume_raycast_intensity: null argument");
-  RMD_REQUIRE(width > 0 && height > 0, "rmd_volume_raycast_intensity: bad image size");
-  RMD_REQUIRE(depth_pitch_ok(depth_pitch, width), "rmd_volume_raycast_intensity: bad depth pitch");
-  RMD_REQUIRE(depth_pitch_ok(intensity_pitch, width), "rmd_volume_raycast_intensity: bad intensity pitch");
-  if(!v->col)
-    return no_intensity("rmd_volume_raycast_intensity");
-  DeviceGuard guard(v->device);
-  VolumeRaycastIntensityParams P;
-  memset(&P, 0, sizeof(P));
-  P.r.g = v->g;
-  P.r.width = width; P.r.height = height;
-  P.r.cam.fx = fx; P.r.cam.fy = fy; P.r.cam.cx = cx; P.r.cam.cy = cy;
-  P.r.T_world_curr = pose_inverse(pose_from(T_curr_world));
-  P.r.depth = dev_depth; P.r.depth_stride = depth_pitch / sizeof(float);
-  P.col = v->col;
-  P.intensity = dev_intensity; P.intensity_stride = intensity_pitch / sizeof(float);
-  RMD_CUDA_TRY(launch_volume_raycast_intensity(P, v->stream));
-  v->n_total += 1;
-  return 0;
-}
-
-int rmd_volume_download_intensity(rmd_volume_t *v, float *host_intensity, float *host_weight)
-{
-  RMD_REQUIRE(v && host_intensity && host_weight, "rmd_volume_download_intensity: null argument");
-  if(!v->col)
-    return no_intensity("rmd_volume_download_intensity");
-  DeviceGuard guard(v->device);
-  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
-  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
-  if(!tmp) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_download_intensity: host allocation failed");
-  cudaError_t err = cudaSuccess;
-  for(size_t b = 0; b < v->n_vox && err == cudaSuccess; b += chunk)
-  {
-    const size_t m = v->n_vox - b < chunk ? v->n_vox - b : chunk;
-    err = cudaMemcpyAsync(tmp, v->col + b, sizeof(float2) * m, cudaMemcpyDeviceToHost, v->stream);
-    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);
-    for(size_t q = 0; q < m && err == cudaSuccess; ++q)
-    {
-      host_intensity[b + q] = tmp[q].x;
-      host_weight[b + q] = tmp[q].y;
-    }
-  }
-  free(tmp);
-  RMD_CUDA_TRY(err);
-  return 0;
-}
-
-int rmd_volume_upload_intensity(rmd_volume_t *v, const float *host_intensity, const float *host_weight)
-{
-  RMD_REQUIRE(v && host_intensity && host_weight, "rmd_volume_upload_intensity: null argument");
-  if(!v->col)
-    return no_intensity("rmd_volume_upload_intensity");
-  DeviceGuard guard(v->device);
-  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
-  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
-  if(!tmp) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_upload_intensity: host allocation failed");
-  cudaError_t err = cudaSuccess;
-  for(size_t b = 0; b < v->n_vox && err == cudaSuccess; b += chunk)
-  {
-    const size_t m = v->n_vox - b < chunk ? v->n_vox - b : chunk;
-    for(size_t q = 0; q < m; ++q)
-      tmp[q] = make_float2(host_intensity[b + q], host_weight[b + q]);
-    err = cudaMemcpyAsync(v->col + b, tmp, sizeof(float2) * m, cudaMemcpyHostToDevice, v->stream);
-    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);   // tmp is refilled next
-  }
-  free(tmp);
-  RMD_CUDA_TRY(err);
   return 0;
 }
 

@@ -2,8 +2,6 @@
 // raycast reads the few voxels around each ray through the read-only path.
 #include "volume.cuh"
 
-#include <cstring>
-
 #define RMD_MC_STORAGE static __constant__
 #include "mc_table.h"
 
@@ -171,16 +169,17 @@ __device__ __forceinline__ unsigned int grid_voxels(const VolumeGrid &g)
 }
 
 // Block b covers voxels [b * VOLUME_SURF_VOXELS, (b + 1) * VOLUME_SURF_VOXELS), in VOLUME_SURF_ROUNDS rounds of
-// VOLUME_SURF_BLOCK consecutive voxels (one per thread, so that loads coalesce).
-__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_count_kernel(const VolumeSurfaceParams P)
+// VOLUME_SURF_BLOCK consecutive voxels (one per thread, so that loads coalesce).  The block's total of count(n), the
+// outputs of voxel n, goes to B.block_offsets[b].
+template<typename Count>
+__device__ __forceinline__ void count_block(const VolumeBlockOffsets &B, Count count)
 {
   __shared__ unsigned int warp_sum[VOLUME_SURF_BLOCK / 32];
-  const unsigned int n_vox = grid_voxels(P.g);
   const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
   unsigned int c = 0;
 #pragma unroll
   for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
-    c += __popc(surface_cell(P.g, base + r * VOLUME_SURF_BLOCK, n_vox).mask);
+    c += count(base + r * VOLUME_SURF_BLOCK);
   c = __reduce_add_sync(0xffffffffu, c);
   if((threadIdx.x & 31) == 0)
     warp_sum[threadIdx.x >> 5] = c;
@@ -189,13 +188,49 @@ __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_count_kernel
   {
     unsigned int tot = 0;
     for(int w = 0; w < VOLUME_SURF_BLOCK / 32; ++w) tot += warp_sum[w];
-    P.block_offsets[blockIdx.x] = tot;
+    B.block_offsets[blockIdx.x] = tot;
   }
+}
+
+// The slot of this thread's first output in a round of a write pass: rank (the outputs of the block's earlier
+// rounds, from its offset on) + the outputs of the threads before it in the round (a warp shuffle scan, then the
+// warps before it); all = the round's outputs.  The caller syncs the block before warp_off is reused.
+__device__ __forceinline__ unsigned long long round_slot(unsigned long long rank, unsigned int cnt,
+                                                         unsigned int *warp_off, unsigned int &all)
+{
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  unsigned int inc = cnt;
+#pragma unroll
+  for(int off = 1; off < 32; off <<= 1)
+  {
+    const unsigned int up = __shfl_up_sync(0xffffffffu, inc, off);
+    if(lane >= off) inc += up;
+  }
+  if(lane == 31)
+    warp_off[wid] = inc;
+  __syncthreads();
+  unsigned int before = 0;
+  all = 0;
+#pragma unroll
+  for(int w = 0; w < VOLUME_SURF_BLOCK / 32; ++w)
+  {
+    const unsigned int x = warp_off[w];
+    before += (w < wid) ? x : 0u;
+    all += x;
+  }
+  return rank + before + inc - cnt;
+}
+
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_count_kernel(const VolumeSurfaceParams P)
+{
+  const unsigned int n_vox = grid_voxels(P.g);
+  count_block(P.b, [&](unsigned int n) { return (unsigned int)__popc(surface_cell(P.g, n, n_vox).mask); });
 }
 
 // Second level: ONE block turns the block totals (up to 2^31 / VOLUME_SURF_VOXELS = 2^20 of them) into exclusive
 // offsets, VOLUME_SCAN_BLOCK * 8 totals per pass (8 consecutive per thread, then a block-wide scan of the sums).
-__global__ void __launch_bounds__(VOLUME_SCAN_BLOCK) volume_surface_scan_kernel(const VolumeSurfaceParams P)
+// It serves the surface points and the mesh's triangles.
+__global__ void __launch_bounds__(VOLUME_SCAN_BLOCK) volume_surface_scan_kernel(const VolumeBlockOffsets P)
 {
   constexpr int PER = 8;
   __shared__ unsigned long long warp_tot[VOLUME_SCAN_BLOCK / 32];
@@ -259,33 +294,14 @@ template<bool KEYS, bool INTENSITY>
 __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_write_kernel(const VolumeSurfaceParams P)
 {
   __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const unsigned int n_vox = grid_voxels(P.g);
   const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
-  unsigned long long rank = P.block_offsets[blockIdx.x];
+  unsigned long long rank = P.b.block_offsets[blockIdx.x];
   for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
   {
     const SurfaceCell c = surface_cell(P.g, base + r * VOLUME_SURF_BLOCK, n_vox);
-    const unsigned int cnt = __popc(c.mask);
-    unsigned int inc = cnt;
-#pragma unroll
-    for(int off = 1; off < 32; off <<= 1)
-    {
-      const unsigned int up = __shfl_up_sync(0xffffffffu, inc, off);
-      if(lane >= off) inc += up;
-    }
-    if(lane == 31)
-      warp_off[wid] = inc;
-    __syncthreads();
-    unsigned int before = 0, all = 0;
-#pragma unroll
-    for(int w = 0; w < VOLUME_SURF_BLOCK / 32; ++w)
-    {
-      const unsigned int x = warp_off[w];
-      before += (w < wid) ? x : 0u;
-      all += x;
-    }
-    unsigned long long slot = rank + before + inc - cnt;
+    unsigned int all;
+    unsigned long long slot = round_slot(rank, __popc(c.mask), warp_off, all);
 #pragma unroll
     for(int axis = 0; axis < 3; ++axis)
     {
@@ -350,23 +366,8 @@ __device__ __forceinline__ unsigned int mesh_cube(const VolumeGrid &g, unsigned 
 
 __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_mesh_count_kernel(const VolumeMeshParams P)
 {
-  __shared__ unsigned int warp_sum[VOLUME_SURF_BLOCK / 32];
   const unsigned int n_vox = grid_voxels(P.g);
-  const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
-  unsigned int c = 0;
-#pragma unroll
-  for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
-    c += RMD_MC_NTRI[mesh_cube(P.g, base + r * VOLUME_SURF_BLOCK, n_vox)];
-  c = __reduce_add_sync(0xffffffffu, c);
-  if((threadIdx.x & 31) == 0)
-    warp_sum[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if(threadIdx.x == 0)
-  {
-    unsigned int tot = 0;
-    for(int w = 0; w < VOLUME_SURF_BLOCK / 32; ++w) tot += warp_sum[w];
-    P.block_offsets[blockIdx.x] = tot;
-  }
+  count_block(P.b, [&](unsigned int n) { return (unsigned int)RMD_MC_NTRI[mesh_cube(P.g, n, n_vox)]; });
 }
 
 // Index of the surface point on edge e of cube n: binary search for its key among the points of the edge's voxel's
@@ -380,7 +381,7 @@ __device__ __forceinline__ int mesh_vertex(const VolumeMeshParams &P, unsigned i
   const unsigned long long key = 3ull * v + axis;
   const unsigned int b = v / VOLUME_SURF_VOXELS;
   unsigned long long lo = P.point_offsets[b];
-  unsigned long long hi = b + 1 < P.n_blocks ? P.point_offsets[b + 1] : P.point_total[0];
+  unsigned long long hi = b + 1 < P.b.n_blocks ? P.point_offsets[b + 1] : P.point_total[0];
   while(lo < hi)
   {
     const unsigned long long mid = (lo + hi) >> 1;
@@ -393,34 +394,16 @@ __device__ __forceinline__ int mesh_vertex(const VolumeMeshParams &P, unsigned i
 __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_mesh_write_kernel(const VolumeMeshParams P)
 {
   __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const unsigned int n_vox = grid_voxels(P.g);
   const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
-  unsigned long long rank = P.block_offsets[blockIdx.x];
+  unsigned long long rank = P.b.block_offsets[blockIdx.x];
   for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
   {
     const unsigned int n = base + r * VOLUME_SURF_BLOCK;
     const unsigned int cube = mesh_cube(P.g, n, n_vox);
     const unsigned int cnt = RMD_MC_NTRI[cube];
-    unsigned int inc = cnt;
-#pragma unroll
-    for(int off = 1; off < 32; off <<= 1)
-    {
-      const unsigned int up = __shfl_up_sync(0xffffffffu, inc, off);
-      if(lane >= off) inc += up;
-    }
-    if(lane == 31)
-      warp_off[wid] = inc;
-    __syncthreads();
-    unsigned int before = 0, all = 0;
-#pragma unroll
-    for(int w = 0; w < VOLUME_SURF_BLOCK / 32; ++w)
-    {
-      const unsigned int x = warp_off[w];
-      before += (w < wid) ? x : 0u;
-      all += x;
-    }
-    unsigned long long slot = rank + before + inc - cnt;
+    unsigned int all;
+    unsigned long long slot = round_slot(rank, cnt, warp_off, all);
     for(unsigned int q = 0; q < cnt && slot < P.capacity; ++q, ++slot)
     {
       int *t = P.tri + 3 * slot;
@@ -434,32 +417,10 @@ __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_mesh_write_kernel(co
 }
 
 // --------------------------------------------------------------------------------------------- raycast
-// Trilinear intensity at grid coordinates (gx, gy, gz), interpolated in x, then y, then z; -1 if a corner lies
-// outside the grid or has colour weight 0.
-__device__ __forceinline__ float sample_intensity(const VolumeGrid &g, const float2 *col, float gx, float gy, float gz)
-{
-  const float x0 = floorf(gx), y0 = floorf(gy), z0 = floorf(gz);
-  const int i0 = (x0 >= 0.0f && x0 < 2.0e9f) ? (int)x0 : -1;
-  const int j0 = (y0 >= 0.0f && y0 < 2.0e9f) ? (int)y0 : -1;
-  const int k0 = (z0 >= 0.0f && z0 < 2.0e9f) ? (int)z0 : -1;
-  if(i0 < 0 || j0 < 0 || k0 < 0 || i0 + 1 >= g.nx || j0 + 1 >= g.ny || k0 + 1 >= g.nz)
-    return -1.0f;
-  const size_t plane = (size_t)g.nx * g.ny;
-  const float2 *b = col + ((size_t)k0 * g.ny + j0) * g.nx + i0;
-  const float2 c000 = __ldg(b), c100 = __ldg(b + 1), c010 = __ldg(b + g.nx), c110 = __ldg(b + g.nx + 1);
-  const float2 c001 = __ldg(b + plane), c101 = __ldg(b + plane + 1), c011 = __ldg(b + plane + g.nx),
-               c111 = __ldg(b + plane + g.nx + 1);
-  if(c000.y == 0.0f || c100.y == 0.0f || c010.y == 0.0f || c110.y == 0.0f || c001.y == 0.0f || c101.y == 0.0f ||
-     c011.y == 0.0f || c111.y == 0.0f)
-    return -1.0f;
-  const float fx = __fsub_rn(gx, x0), fy = __fsub_rn(gy, y0), fz = __fsub_rn(gz, z0);
-  const float c00 = lerp_rn(c000.x, c100.x, fx), c10 = lerp_rn(c010.x, c110.x, fx);
-  const float c01 = lerp_rn(c001.x, c101.x, fx), c11 = lerp_rn(c011.x, c111.x, fx);
-  return lerp_rn(lerp_rn(c00, c10, fy), lerp_rn(c01, c11, fy), fz);
-}
-
-// Trilinear TSDF at grid coordinates (gx, gy, gz); false if a corner lies outside the grid or is unknown.
-__device__ __forceinline__ bool sample_tsdf(const VolumeGrid &g, float gx, float gy, float gz, float &out)
+// Trilinear interpolation of the records rec (g.vox or the intensity records, indexed alike) at grid coordinates
+// (gx, gy, gz), in x, then y, then z; false if a corner lies outside the grid or has weight 0.
+__device__ __forceinline__ bool sample_records(const VolumeGrid &g, const float2 *rec, float gx, float gy, float gz,
+                                               float &out)
 {
   const float x0 = floorf(gx), y0 = floorf(gy), z0 = floorf(gz);
   const int i0 = (x0 >= 0.0f && x0 < 2.0e9f) ? (int)x0 : -1;
@@ -468,7 +429,7 @@ __device__ __forceinline__ bool sample_tsdf(const VolumeGrid &g, float gx, float
   if(i0 < 0 || j0 < 0 || k0 < 0 || i0 + 1 >= g.nx || j0 + 1 >= g.ny || k0 + 1 >= g.nz)
     return false;
   const size_t plane = (size_t)g.nx * g.ny;
-  const float2 *b = g.vox + ((size_t)k0 * g.ny + j0) * g.nx + i0;
+  const float2 *b = rec + ((size_t)k0 * g.ny + j0) * g.nx + i0;
   const float2 c000 = __ldg(b), c100 = __ldg(b + 1), c010 = __ldg(b + g.nx), c110 = __ldg(b + g.nx + 1);
   const float2 c001 = __ldg(b + plane), c101 = __ldg(b + plane + 1), c011 = __ldg(b + plane + g.nx),
                c111 = __ldg(b + plane + g.nx + 1);
@@ -483,10 +444,9 @@ __device__ __forceinline__ bool sample_tsdf(const VolumeGrid &g, float gx, float
 }
 
 // The ray of pixel (x, y).  INTENSITY: also the intensity at the hit, from the grid coordinates of org + t dir in the
-// march's form, into I (the plain instance ignores col and I).
+// march's form (the plain instance ignores C).
 template<bool INTENSITY>
-__device__ __forceinline__ void raycast_pixel(const VolumeRaycastParams &P, int x, int y, const float2 *col, float *I,
-                                              size_t I_stride)
+__device__ __forceinline__ void raycast_pixel(const VolumeRaycastParams &P, const VolumeRaycastColour &C, int x, int y)
 {
   const VolumeGrid &g = P.g;
   // the ray of back_project (point_cloud.cuh), rotated into the world; it starts at the camera centre
@@ -537,14 +497,15 @@ __device__ __forceinline__ void raycast_pixel(const VolumeRaycastParams &P, int 
       const float gy = __fdiv_rn(__fsub_rn(__fadd_rn(org[1], __fmul_rn(t, dir[1])), g.oy), s);
       const float gz = __fdiv_rn(__fsub_rn(__fadd_rn(org[2], __fmul_rn(t, dir[2])), g.oz), s);
       float f = 0.0f;
-      const bool known = sample_tsdf(g, gx, gy, gz, f);
+      const bool known = sample_records(g, g.vox, gx, gy, gz, f);
       if(known && prev_known && f_prev > 0.0f && f <= 0.0f)
       {
         out = __fadd_rn(t_prev, __fdiv_rn(__fmul_rn(s, f_prev), __fsub_rn(f_prev, f)));
-        if(INTENSITY)
-          inten = sample_intensity(g, col, __fdiv_rn(__fsub_rn(__fadd_rn(org[0], __fmul_rn(out, dir[0])), g.ox), s),
-                                   __fdiv_rn(__fsub_rn(__fadd_rn(org[1], __fmul_rn(out, dir[1])), g.oy), s),
-                                   __fdiv_rn(__fsub_rn(__fadd_rn(org[2], __fmul_rn(out, dir[2])), g.oz), s));
+        if(INTENSITY &&
+           !sample_records(g, C.col, __fdiv_rn(__fsub_rn(__fadd_rn(org[0], __fmul_rn(out, dir[0])), g.ox), s),
+                           __fdiv_rn(__fsub_rn(__fadd_rn(org[1], __fmul_rn(out, dir[1])), g.oy), s),
+                           __fdiv_rn(__fsub_rn(__fadd_rn(org[2], __fmul_rn(out, dir[2])), g.oz), s), inten))
+          inten = -1.0f;
         break;
       }
       prev_known = known;
@@ -554,25 +515,19 @@ __device__ __forceinline__ void raycast_pixel(const VolumeRaycastParams &P, int 
   }
   P.depth[(size_t)y * P.depth_stride + x] = out;
   if(INTENSITY)
-    I[(size_t)y * I_stride + x] = inten;
+    C.intensity[(size_t)y * C.intensity_stride + x] = inten;
 }
 
-__global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycastParams P)
+// The colour fields are a parameter of their own: past 128 B a parameter is read through a pointer, which slows the
+// plain rays by about 5 %.
+template<bool INTENSITY>
+__global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycastParams P, const VolumeRaycastColour C)
 {
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
   const int y = blockIdx.y * blockDim.y + threadIdx.y;
   if(x >= P.width || y >= P.height)
     return;
-  raycast_pixel<false>(P, x, y, nullptr, nullptr, 0);
-}
-
-__global__ void __launch_bounds__(256) volume_raycast_intensity_kernel(const VolumeRaycastIntensityParams P)
-{
-  const int x = blockIdx.x * blockDim.x + threadIdx.x;
-  const int y = blockIdx.y * blockDim.y + threadIdx.y;
-  if(x >= P.r.width || y >= P.r.height)
-    return;
-  raycast_pixel<true>(P.r, x, y, P.col, P.intensity, P.intensity_stride);
+  raycast_pixel<INTENSITY>(P, C, x, y);
 }
 
 } // namespace
@@ -589,65 +544,47 @@ cudaError_t launch_volume_integrate(const VolumeIntegrateParams &P, cudaStream_t
 
 cudaError_t launch_volume_surface_count(const VolumeSurfaceParams &P, cudaStream_t stream)
 {
-  volume_surface_count_kernel<<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  volume_surface_count_kernel<<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   cudaError_t err = cudaGetLastError();
   if(err != cudaSuccess) return err;
-  volume_surface_scan_kernel<<<1, VOLUME_SCAN_BLOCK, 0, stream>>>(P);
+  volume_surface_scan_kernel<<<1, VOLUME_SCAN_BLOCK, 0, stream>>>(P.b);
   return cudaGetLastError();
 }
 
 cudaError_t launch_volume_surface_write(const VolumeSurfaceParams &P, cudaStream_t stream)
 {
-  volume_surface_write_kernel<false, false><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_volume_surface_write_keys(const VolumeSurfaceParams &P, cudaStream_t stream)
-{
-  volume_surface_write_kernel<true, false><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_volume_surface_write_intensity(const VolumeSurfaceParams &P, cudaStream_t stream)
-{
-  volume_surface_write_kernel<false, true><<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  if(P.keys)
+    volume_surface_write_kernel<true, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  else if(P.intensity)
+    volume_surface_write_kernel<false, true><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  else
+    volume_surface_write_kernel<false, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   return cudaGetLastError();
 }
 
 cudaError_t launch_volume_mesh_count(const VolumeMeshParams &P, cudaStream_t stream)
 {
-  volume_mesh_count_kernel<<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  volume_mesh_count_kernel<<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   cudaError_t err = cudaGetLastError();
   if(err != cudaSuccess) return err;
-  VolumeSurfaceParams S;   // the surface points' block-total scan, on the triangle totals
-  memset(&S, 0, sizeof(S));
-  S.g = P.g;
-  S.block_offsets = P.block_offsets;
-  S.total = P.total;
-  S.n_blocks = P.n_blocks;
-  volume_surface_scan_kernel<<<1, VOLUME_SCAN_BLOCK, 0, stream>>>(S);
+  volume_surface_scan_kernel<<<1, VOLUME_SCAN_BLOCK, 0, stream>>>(P.b);
   return cudaGetLastError();
 }
 
 cudaError_t launch_volume_mesh_write(const VolumeMeshParams &P, cudaStream_t stream)
 {
-  volume_mesh_write_kernel<<<P.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  volume_mesh_write_kernel<<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   return cudaGetLastError();
 }
 
-cudaError_t launch_volume_raycast(const VolumeRaycastParams &P, cudaStream_t stream)
+cudaError_t launch_volume_raycast(const VolumeRaycastParams &P, const VolumeRaycastColour &C, cudaStream_t stream)
 {
   const dim3 block(32, 8);
   const dim3 grid((P.width + block.x - 1) / block.x, (P.height + block.y - 1) / block.y);
-  volume_raycast_kernel<<<grid, block, 0, stream>>>(P);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_volume_raycast_intensity(const VolumeRaycastIntensityParams &P, cudaStream_t stream)
-{
-  const dim3 block(32, 8);
-  const dim3 grid((P.r.width + block.x - 1) / block.x, (P.r.height + block.y - 1) / block.y);
-  volume_raycast_intensity_kernel<<<grid, block, 0, stream>>>(P);
+  if(C.col)
+    volume_raycast_kernel<true><<<grid, block, 0, stream>>>(P, C);
+  else
+    volume_raycast_kernel<false><<<grid, block, 0, stream>>>(P, C);
   return cudaGetLastError();
 }
 

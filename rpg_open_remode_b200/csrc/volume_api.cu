@@ -1,0 +1,540 @@
+// volume_api.cu -- the C-ABI of the TSDF volume (rmd_volume_*, include/rmd_b200.h; DESIGN.md 4.8): the handle,
+// argument checks, scratch and staging buffers, and the host sequencing of the kernels in volume.cu.
+// rmd_volume_integrate_seeds is in c_api.cu, next to the seeds' internals it reads.
+#include <math.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include <new>
+#include <string>
+
+#include "rmd_common.cuh"
+#include "volume.cuh"
+
+namespace rmdb
+{
+
+int volume_integrate(rmd_volume *v, VolumeIntegrateParams &P)
+{
+  P.g = v->g;
+  P.trunc = v->trunc; P.max_weight = v->max_weight;
+  P.col = P.intensity ? v->col : NULL;
+  RMD_CUDA_TRY(launch_volume_integrate(P, v->stream));
+  return 0;
+}
+
+} // namespace rmdb
+
+using namespace rmdb;
+
+namespace
+{
+
+const size_t kVolumeMaxVoxels = (size_t)1 << 31;
+const size_t kVolumeChunk = (size_t)1 << 24;   // voxels per host staging chunk of download / upload
+
+// Argument check of an entry point whose name is `what`.
+#define VOLUME_REQUIRE(cond, msg)                                                                  \
+  do {                                                                                             \
+    if(!(cond))                                                                                    \
+      return fail(RMD_ERR_INVALID_ARGUMENT, (std::string(what) + ": " + (msg)).c_str());           \
+  } while(0)
+
+int no_intensity(const char *what)
+{
+  return fail(RMD_ERR_NOT_INITIALISED, (std::string(what) + ": the volume has no intensity channel").c_str());
+}
+
+// Device buffer of at least n elements, grown (never shrunk) on demand.
+template<typename T>
+int volume_grow(T **buf, size_t *cap, size_t n)
+{
+  if(n <= *cap)
+    return 0;
+  RMD_CUDA_TRY(cudaFree(*buf));
+  *buf = NULL; *cap = 0;
+  RMD_CUDA_TRY(cudaMalloc(buf, sizeof(T) * n));
+  *cap = n;
+  return 0;
+}
+
+// The surface points' pass parameters on v's grid, with the per-block offsets and total (allocated on first use).
+int volume_surface_params(rmd_volume *v, VolumeSurfaceParams &P)
+{
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.b.n_blocks = (unsigned int)((v->n_vox + VOLUME_SURF_VOXELS - 1) / VOLUME_SURF_VOXELS);
+  if(!v->surf_offsets)
+  {
+    RMD_CUDA_TRY(cudaMalloc(&v->surf_offsets, sizeof(unsigned long long) * P.b.n_blocks));
+    RMD_CUDA_TRY(cudaMalloc(&v->surf_total, sizeof(unsigned long long)));
+  }
+  P.b.block_offsets = v->surf_offsets;
+  P.b.total = v->surf_total;
+  return 0;
+}
+
+// The surface points' count pass and scan, one host read of the count, then for min(count, capacity) points their
+// write pass: positions (float4), or with intensity every point's intensity (float, same blocks and ranks).  host:
+// staged in v->stage and copied to out.  Synchronous.
+int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, bool host, bool intensity)
+{
+  VolumeSurfaceParams P;
+  int rc = volume_surface_params(v, P);
+  if(rc) return rc;
+  RMD_CUDA_TRY(launch_volume_surface_count(P, v->stream));
+  unsigned long long total = 0;
+  RMD_CUDA_TRY(cudaMemcpyAsync(&total, v->surf_total, sizeof(total), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  *count = (size_t)total;
+  const size_t n = *count < capacity ? *count : capacity;
+  if(!n)
+    return 0;
+  const size_t bytes = n * (intensity ? sizeof(float) : sizeof(float4));
+  void *dst = out;
+  if(host)
+  {
+    rc = volume_grow(&v->stage, &v->stage_cap, bytes);
+    if(rc) return rc;
+    dst = v->stage;
+  }
+  P.capacity = n;
+  if(intensity)
+  {
+    P.col = v->col;
+    P.intensity = static_cast<float*>(dst);
+  }
+  else
+    P.out = static_cast<float4*>(dst);
+  RMD_CUDA_TRY(launch_volume_surface_write(P, v->stream));
+  if(host)
+    RMD_CUDA_TRY(cudaMemcpyAsync(out, v->stage, bytes, cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  return 0;
+}
+
+// The mesh: both count passes and scans, one host read of the two totals, then -- for what the capacities ask --
+// the surface points (with their keys when triangles are wanted) and the triangles.  host: min(count, capacity)
+// of each are staged in the volume's buffers and copied to xyzw / tri.  Synchronous.
+int volume_mesh(rmd_volume *v, void *xyzw, size_t vertex_capacity, int32_t *tri, size_t tri_capacity,
+                size_t *n_vertices, size_t *n_triangles, bool host, const char *what)
+{
+  VolumeSurfaceParams S;
+  int rc = volume_surface_params(v, S);
+  if(rc) return rc;
+  if(!v->tri_offsets)
+  {
+    RMD_CUDA_TRY(cudaMalloc(&v->tri_offsets, sizeof(unsigned long long) * S.b.n_blocks));
+    RMD_CUDA_TRY(cudaMalloc(&v->tri_total, sizeof(unsigned long long)));
+  }
+  VolumeMeshParams M;
+  memset(&M, 0, sizeof(M));
+  M.g = v->g;
+  M.point_offsets = v->surf_offsets;
+  M.point_total = v->surf_total;
+  M.b.block_offsets = v->tri_offsets;
+  M.b.total = v->tri_total;
+  M.b.n_blocks = S.b.n_blocks;
+  RMD_CUDA_TRY(launch_volume_surface_count(S, v->stream));
+  RMD_CUDA_TRY(launch_volume_mesh_count(M, v->stream));
+  unsigned long long nv = 0, nt = 0;
+  RMD_CUDA_TRY(cudaMemcpyAsync(&nv, v->surf_total, sizeof(nv), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaMemcpyAsync(&nt, v->tri_total, sizeof(nt), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  *n_vertices = (size_t)nv;
+  *n_triangles = (size_t)nt;
+  if(nv >= (1ull << 31))
+    return fail(RMD_ERR_UNSUPPORTED, (std::string(what) + ": 2^31 or more vertices do not fit int32 indices").c_str());
+  const size_t mv = nv < vertex_capacity ? (size_t)nv : vertex_capacity;
+  const size_t mt = nt < tri_capacity ? (size_t)nt : tri_capacity;
+  if(!mv && !mt)
+    return 0;
+  float4 *vout = reinterpret_cast<float4*>(xyzw);
+  int *tout = tri;
+  if(host)
+  {
+    rc = volume_grow(&v->stage, &v->stage_cap, mv * sizeof(float4));
+    if(!rc) rc = volume_grow(&v->tri_stage, &v->tri_stage_cap, 3 * mt);
+    if(rc) return rc;
+    vout = reinterpret_cast<float4*>(v->stage);
+    tout = v->tri_stage;
+  }
+  S.out = vout;
+  S.capacity = mv;
+  if(mt)
+  {
+    // every vertex's key, whatever the vertex capacity: triangles may index vertices that are not returned
+    rc = volume_grow(&v->keys, &v->keys_cap, (size_t)nv);
+    if(rc) return rc;
+    S.keys = v->keys;
+  }
+  RMD_CUDA_TRY(launch_volume_surface_write(S, v->stream));
+  if(mt)
+  {
+    M.keys = v->keys;
+    M.tri = tout;
+    M.capacity = mt;
+    RMD_CUDA_TRY(launch_volume_mesh_write(M, v->stream));
+  }
+  if(host)
+  {
+    if(mv)
+      RMD_CUDA_TRY(cudaMemcpyAsync(xyzw, v->stage, mv * sizeof(float4), cudaMemcpyDeviceToHost, v->stream));
+    if(mt)
+      RMD_CUDA_TRY(cudaMemcpyAsync(tri, v->tri_stage, mt * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, v->stream));
+  }
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  return 0;
+}
+
+// rmd_volume_integrate_depth[_intensity]: with_intensity also requires and fuses the image.
+int volume_integrate_depth(const char *what, rmd_volume_t *v, int width, int height, float fx, float fy, float cx,
+                           float cy, const float *T_curr_world, const float *dev_depth, size_t depth_pitch,
+                           const int32_t *dev_conv, size_t conv_pitch, bool with_intensity,
+                           const float *dev_intensity, size_t intensity_pitch)
+{
+  VOLUME_REQUIRE(v && T_curr_world && dev_depth && (!with_intensity || dev_intensity), "null argument");
+  VOLUME_REQUIRE(width > 0 && height > 0, "bad image size");
+  VOLUME_REQUIRE(depth_pitch_ok(depth_pitch, width), "bad depth pitch");
+  VOLUME_REQUIRE(!dev_conv || (conv_pitch >= sizeof(int32_t) * (size_t)width && conv_pitch % sizeof(int32_t) == 0),
+                 "bad state pitch");
+  if(with_intensity)
+  {
+    VOLUME_REQUIRE(depth_pitch_ok(intensity_pitch, width), "bad intensity pitch");
+    if(!v->col)
+      return no_intensity(what);
+  }
+  DeviceGuard guard(v->device);
+  VolumeIntegrateParams P;
+  memset(&P, 0, sizeof(P));
+  P.width = width; P.height = height;
+  P.cam.fx = fx; P.cam.fy = fy; P.cam.cx = cx; P.cam.cy = cy;
+  P.T_curr_world = pose_from(T_curr_world);
+  P.depth = dev_depth; P.depth_stride = depth_pitch / sizeof(float); P.depth_comps = 1;
+  P.conv = dev_conv; P.conv_stride = conv_pitch / sizeof(int32_t);
+  if(with_intensity)
+  {
+    P.intensity = dev_intensity; P.intensity_stride = intensity_pitch / sizeof(float);
+  }
+  return volume_integrate(v, P);
+}
+
+// rmd_volume_raycast[_intensity]: with_intensity also requires and writes the intensity image.
+int volume_raycast(const char *what, rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                   const float *T_curr_world, float *dev_depth, size_t depth_pitch, bool with_intensity,
+                   float *dev_intensity, size_t intensity_pitch)
+{
+  VOLUME_REQUIRE(v && T_curr_world && dev_depth && (!with_intensity || dev_intensity), "null argument");
+  VOLUME_REQUIRE(width > 0 && height > 0, "bad image size");
+  VOLUME_REQUIRE(depth_pitch_ok(depth_pitch, width), "bad depth pitch");
+  if(with_intensity)
+  {
+    VOLUME_REQUIRE(depth_pitch_ok(intensity_pitch, width), "bad intensity pitch");
+    if(!v->col)
+      return no_intensity(what);
+  }
+  DeviceGuard guard(v->device);
+  VolumeRaycastParams P;
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.width = width; P.height = height;
+  P.cam.fx = fx; P.cam.fy = fy; P.cam.cx = cx; P.cam.cy = cy;
+  P.T_world_curr = pose_inverse(pose_from(T_curr_world));
+  P.depth = dev_depth; P.depth_stride = depth_pitch / sizeof(float);
+  VolumeRaycastColour C;
+  memset(&C, 0, sizeof(C));
+  if(with_intensity)
+  {
+    C.col = v->col;
+    C.intensity = dev_intensity; C.intensity_stride = intensity_pitch / sizeof(float);
+  }
+  RMD_CUDA_TRY(launch_volume_raycast(P, C, v->stream));
+  return 0;
+}
+
+// A record array (g.vox or col) to two host arrays of n_vox floats (.x to a, .y to b), through host chunks.
+int volume_download_records(rmd_volume *v, const float2 *records, float *a, float *b, const char *what)
+{
+  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
+  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
+  if(!tmp) return fail((int)cudaErrorMemoryAllocation, (std::string(what) + ": host allocation failed").c_str());
+  cudaError_t err = cudaSuccess;
+  for(size_t c = 0; c < v->n_vox && err == cudaSuccess; c += chunk)
+  {
+    const size_t m = v->n_vox - c < chunk ? v->n_vox - c : chunk;
+    err = cudaMemcpyAsync(tmp, records + c, sizeof(float2) * m, cudaMemcpyDeviceToHost, v->stream);
+    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);
+    for(size_t q = 0; q < m && err == cudaSuccess; ++q)
+    {
+      a[c + q] = tmp[q].x;
+      b[c + q] = tmp[q].y;
+    }
+  }
+  free(tmp);
+  RMD_CUDA_TRY(err);
+  return 0;
+}
+
+// The inverse: two host arrays joined into the record array.
+int volume_upload_records(rmd_volume *v, float2 *records, const float *a, const float *b, const char *what)
+{
+  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
+  float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
+  if(!tmp) return fail((int)cudaErrorMemoryAllocation, (std::string(what) + ": host allocation failed").c_str());
+  cudaError_t err = cudaSuccess;
+  for(size_t c = 0; c < v->n_vox && err == cudaSuccess; c += chunk)
+  {
+    const size_t m = v->n_vox - c < chunk ? v->n_vox - c : chunk;
+    for(size_t q = 0; q < m; ++q)
+      tmp[q] = make_float2(a[c + q], b[c + q]);
+    err = cudaMemcpyAsync(records + c, tmp, sizeof(float2) * m, cudaMemcpyHostToDevice, v->stream);
+    if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);   // tmp is refilled next
+  }
+  free(tmp);
+  RMD_CUDA_TRY(err);
+  return 0;
+}
+
+} // namespace
+
+extern "C"
+{
+
+int rmd_volume_create(int nx, int ny, int nz, float voxel_size, const float origin[3], float truncation,
+                      float max_weight, int device, rmd_volume_t **out)
+{
+  RMD_REQUIRE(out, "rmd_volume_create: out is null");
+  *out = NULL;
+  RMD_REQUIRE(origin, "rmd_volume_create: origin is null");
+  RMD_REQUIRE(nx > 0 && ny > 0 && nz > 0, "rmd_volume_create: grid dimensions must be positive");
+  const uint64_t plane = (uint64_t)nx * (uint64_t)ny;   // each factor < 2^31: no overflow in 64 bits
+  RMD_REQUIRE(plane <= kVolumeMaxVoxels && plane * (uint64_t)nz <= kVolumeMaxVoxels,
+              "rmd_volume_create: at most 2^31 voxels");
+  RMD_REQUIRE(voxel_size > 0.0f && isfinite(voxel_size), "rmd_volume_create: voxel_size must be > 0");
+  RMD_REQUIRE(truncation > 0.0f && isfinite(truncation), "rmd_volume_create: truncation must be > 0");
+  RMD_REQUIRE(max_weight >= 1.0f, "rmd_volume_create: max_weight must be >= 1");
+  RMD_REQUIRE(isfinite(origin[0]) && isfinite(origin[1]) && isfinite(origin[2]), "rmd_volume_create: bad origin");
+  if(device < 0) RMD_CUDA_TRY(cudaGetDevice(&device));
+  DeviceGuard guard(device);
+  rmd_volume *v = new(std::nothrow) rmd_volume();
+  if(!v) return fail((int)cudaErrorMemoryAllocation, "rmd_volume_create: host allocation failed");
+  memset(v, 0, sizeof(*v));
+  v->device = device;
+  v->g.nx = nx; v->g.ny = ny; v->g.nz = nz;
+  v->g.voxel = voxel_size;
+  v->g.ox = origin[0]; v->g.oy = origin[1]; v->g.oz = origin[2];
+  v->n_vox = (size_t)(plane * (uint64_t)nz);
+  v->trunc = truncation; v->max_weight = max_weight;
+  cudaError_t err = cudaStreamCreateWithFlags(&v->own_stream, cudaStreamNonBlocking);
+  if(err == cudaSuccess) err = cudaEventCreateWithFlags(&v->seeds_ev, cudaEventDisableTiming);
+  if(err == cudaSuccess) err = cudaMalloc(&v->g.vox, sizeof(float2) * v->n_vox);
+  if(err == cudaSuccess) err = cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->own_stream);
+  if(err == cudaSuccess) err = cudaStreamSynchronize(v->own_stream);
+  if(err != cudaSuccess)
+  {
+    rmd_volume_destroy(v);
+    return fail_cuda(err, "rmd_volume_create");
+  }
+  v->stream = v->own_stream;
+  *out = v;
+  return 0;
+}
+
+int rmd_volume_destroy(rmd_volume_t *v)
+{
+  if(!v) return 0;
+  DeviceGuard guard(v->device);
+  cudaDeviceSynchronize();
+  if(v->own_stream) cudaStreamDestroy(v->own_stream);
+  if(v->seeds_ev) cudaEventDestroy(v->seeds_ev);
+  cudaFree(v->g.vox);
+  cudaFree(v->surf_offsets); cudaFree(v->surf_total); cudaFree(v->stage);
+  cudaFree(v->tri_offsets); cudaFree(v->tri_total); cudaFree(v->keys); cudaFree(v->tri_stage);
+  cudaFree(v->col);
+  cudaGetLastError();
+  delete v;
+  return 0;
+}
+
+int rmd_volume_set_stream(rmd_volume_t *v, void *cuda_stream)
+{
+  RMD_REQUIRE(v, "rmd_volume_set_stream: null handle");
+  DeviceGuard guard(v->device);
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  v->stream = cuda_stream ? (cudaStream_t)cuda_stream : v->own_stream;
+  return 0;
+}
+
+int rmd_volume_reset(rmd_volume_t *v)
+{
+  RMD_REQUIRE(v, "rmd_volume_reset: null handle");
+  DeviceGuard guard(v->device);
+  RMD_CUDA_TRY(cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->stream));
+  if(v->col)
+    RMD_CUDA_TRY(cudaMemsetAsync(v->col, 0, sizeof(float2) * v->n_vox, v->stream));
+  return 0;
+}
+
+int rmd_volume_sync(rmd_volume_t *v)
+{
+  RMD_REQUIRE(v, "rmd_volume_sync: null handle");
+  DeviceGuard guard(v->device);
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  return 0;
+}
+
+int rmd_volume_size(rmd_volume_t *v, int *nx, int *ny, int *nz, float *voxel_size, float origin[3])
+{
+  RMD_REQUIRE(v, "rmd_volume_size: null handle");
+  if(nx) *nx = v->g.nx;
+  if(ny) *ny = v->g.ny;
+  if(nz) *nz = v->g.nz;
+  if(voxel_size) *voxel_size = v->g.voxel;
+  if(origin) { origin[0] = v->g.ox; origin[1] = v->g.oy; origin[2] = v->g.oz; }
+  return 0;
+}
+
+int rmd_volume_enable_intensity(rmd_volume_t *v)
+{
+  RMD_REQUIRE(v, "rmd_volume_enable_intensity: null handle");
+  if(v->col)
+    return 0;
+  DeviceGuard guard(v->device);
+  cudaError_t err = cudaMalloc(&v->col, sizeof(float2) * v->n_vox);
+  if(err != cudaSuccess)
+  {
+    v->col = NULL;
+    return fail_cuda(err, "rmd_volume_enable_intensity");
+  }
+  err = cudaMemsetAsync(v->col, 0, sizeof(float2) * v->n_vox, v->stream);
+  if(err != cudaSuccess)
+  {
+    cudaFree(v->col);
+    v->col = NULL;
+    return fail_cuda(err, "rmd_volume_enable_intensity");
+  }
+  return 0;
+}
+
+int rmd_volume_integrate_depth(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                               const float *T_curr_world, const float *dev_depth, size_t depth_pitch,
+                               const int32_t *dev_conv, size_t conv_pitch)
+{
+  return volume_integrate_depth("rmd_volume_integrate_depth", v, width, height, fx, fy, cx, cy, T_curr_world,
+                                dev_depth, depth_pitch, dev_conv, conv_pitch, false, NULL, 0);
+}
+
+int rmd_volume_integrate_depth_intensity(rmd_volume_t *v, int width, int height, float fx, float fy, float cx,
+                                         float cy, const float *T_curr_world, const float *dev_depth,
+                                         size_t depth_pitch, const int32_t *dev_conv, size_t conv_pitch,
+                                         const float *dev_intensity, size_t intensity_pitch)
+{
+  return volume_integrate_depth("rmd_volume_integrate_depth_intensity", v, width, height, fx, fy, cx, cy,
+                                T_curr_world, dev_depth, depth_pitch, dev_conv, conv_pitch, true, dev_intensity,
+                                intensity_pitch);
+}
+
+int rmd_volume_surface_points(rmd_volume_t *v, float *host_xyzw, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (host_xyzw || capacity == 0), "rmd_volume_surface_points: null argument");
+  DeviceGuard guard(v->device);
+  return volume_surface(v, host_xyzw, capacity, count, true, false);
+}
+
+int rmd_volume_surface_points_device(rmd_volume_t *v, float *dev_xyzw, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (dev_xyzw || capacity == 0), "rmd_volume_surface_points_device: null argument");
+  RMD_REQUIRE(((uintptr_t)dev_xyzw % 16) == 0, "rmd_volume_surface_points_device: output must be 16-byte aligned");
+  DeviceGuard guard(v->device);
+  return volume_surface(v, dev_xyzw, capacity, count, false, false);
+}
+
+int rmd_volume_surface_intensity(rmd_volume_t *v, float *host_intensity, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (host_intensity || capacity == 0), "rmd_volume_surface_intensity: null argument");
+  if(!v->col)
+    return no_intensity("rmd_volume_surface_intensity");
+  DeviceGuard guard(v->device);
+  return volume_surface(v, host_intensity, capacity, count, true, true);
+}
+
+int rmd_volume_surface_intensity_device(rmd_volume_t *v, float *dev_intensity, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (dev_intensity || capacity == 0), "rmd_volume_surface_intensity_device: null argument");
+  RMD_REQUIRE(((uintptr_t)dev_intensity % 4) == 0, "rmd_volume_surface_intensity_device: output must be 4-byte aligned");
+  if(!v->col)
+    return no_intensity("rmd_volume_surface_intensity_device");
+  DeviceGuard guard(v->device);
+  return volume_surface(v, dev_intensity, capacity, count, false, true);
+}
+
+int rmd_volume_mesh(rmd_volume_t *v, float *host_xyzw, size_t vertex_capacity, int32_t *host_tri,
+                    size_t tri_capacity, size_t *n_vertices, size_t *n_triangles)
+{
+  RMD_REQUIRE(v && n_vertices && n_triangles && (host_xyzw || vertex_capacity == 0) && (host_tri || tri_capacity == 0),
+              "rmd_volume_mesh: null argument");
+  DeviceGuard guard(v->device);
+  return volume_mesh(v, host_xyzw, vertex_capacity, host_tri, tri_capacity, n_vertices, n_triangles, true,
+                     "rmd_volume_mesh");
+}
+
+int rmd_volume_mesh_device(rmd_volume_t *v, float *dev_xyzw, size_t vertex_capacity, int32_t *dev_tri,
+                           size_t tri_capacity, size_t *n_vertices, size_t *n_triangles)
+{
+  RMD_REQUIRE(v && n_vertices && n_triangles && (dev_xyzw || vertex_capacity == 0) && (dev_tri || tri_capacity == 0),
+              "rmd_volume_mesh_device: null argument");
+  RMD_REQUIRE(((uintptr_t)dev_xyzw % 16) == 0, "rmd_volume_mesh_device: vertices must be 16-byte aligned");
+  RMD_REQUIRE(((uintptr_t)dev_tri % 4) == 0, "rmd_volume_mesh_device: triangles must be 4-byte aligned");
+  DeviceGuard guard(v->device);
+  return volume_mesh(v, dev_xyzw, vertex_capacity, dev_tri, tri_capacity, n_vertices, n_triangles, false,
+                     "rmd_volume_mesh_device");
+}
+
+int rmd_volume_raycast(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                       const float *T_curr_world, float *dev_depth, size_t depth_pitch)
+{
+  return volume_raycast("rmd_volume_raycast", v, width, height, fx, fy, cx, cy, T_curr_world, dev_depth, depth_pitch,
+                        false, NULL, 0);
+}
+
+int rmd_volume_raycast_intensity(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                                 const float *T_curr_world, float *dev_depth, size_t depth_pitch,
+                                 float *dev_intensity, size_t intensity_pitch)
+{
+  return volume_raycast("rmd_volume_raycast_intensity", v, width, height, fx, fy, cx, cy, T_curr_world, dev_depth,
+                        depth_pitch, true, dev_intensity, intensity_pitch);
+}
+
+int rmd_volume_download(rmd_volume_t *v, float *host_tsdf, float *host_weight)
+{
+  RMD_REQUIRE(v && host_tsdf && host_weight, "rmd_volume_download: null argument");
+  DeviceGuard guard(v->device);
+  return volume_download_records(v, v->g.vox, host_tsdf, host_weight, "rmd_volume_download");
+}
+
+int rmd_volume_upload(rmd_volume_t *v, const float *host_tsdf, const float *host_weight)
+{
+  RMD_REQUIRE(v && host_tsdf && host_weight, "rmd_volume_upload: null argument");
+  DeviceGuard guard(v->device);
+  return volume_upload_records(v, v->g.vox, host_tsdf, host_weight, "rmd_volume_upload");
+}
+
+int rmd_volume_download_intensity(rmd_volume_t *v, float *host_intensity, float *host_weight)
+{
+  RMD_REQUIRE(v && host_intensity && host_weight, "rmd_volume_download_intensity: null argument");
+  if(!v->col)
+    return no_intensity("rmd_volume_download_intensity");
+  DeviceGuard guard(v->device);
+  return volume_download_records(v, v->col, host_intensity, host_weight, "rmd_volume_download_intensity");
+}
+
+int rmd_volume_upload_intensity(rmd_volume_t *v, const float *host_intensity, const float *host_weight)
+{
+  RMD_REQUIRE(v && host_intensity && host_weight, "rmd_volume_upload_intensity: null argument");
+  if(!v->col)
+    return no_intensity("rmd_volume_upload_intensity");
+  DeviceGuard guard(v->device);
+  return volume_upload_records(v, v->col, host_intensity, host_weight, "rmd_volume_upload_intensity");
+}
+
+} // extern "C"
