@@ -85,6 +85,16 @@ public:
                            "TsdfVolume: unable to raycast");
   }
 
+  // Right after seeds.setReferenceImage (no update since): the new keyframe's depth prior from the fused model --
+  // every non-BORDER pixel whose ray hits the surface within the seeds' depth range gets (hit, sigma_sq_frac *
+  // range^2 / 36, 10, 10); the other seeds are left as they are.  Asynchronous, ordered after the volume's queued
+  // work.
+  void seedPrior(SeedMatrix &seeds, float sigma_sq_frac)
+  {
+    detail::throw_on_error(rmd_volume_prior_seeds(handle_, seeds.handle(), sigma_sq_frac),
+                           "TsdfVolume: unable to seed the keyframe prior");
+  }
+
   // Intensity channel (8 B per voxel): from now on integrate() also fuses the keyframe's reference image.
   void enableIntensity()
   {

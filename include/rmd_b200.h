@@ -506,6 +506,27 @@ int rmd_volume_mesh_device(rmd_volume_t *v, float *dev_xyzw, size_t vertex_capac
 int rmd_volume_raycast(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
                        const float *T_curr_world, float *dev_depth, size_t depth_pitch);
 
+/* Depth prior of a new keyframe from the fused model (DESIGN.md 4.8): s has
+ * just had set_reference* and no update since.  Every non-BORDER pixel of s is
+ * raycast as rmd_volume_raycast does with s's camera and the pose its
+ * reference was set with; a hit d with min_depth <= d <= max_depth (s's)
+ * becomes the seed (d, sigma_sq_frac * range^2 / 36, 10, 10), d bit-identical
+ * to rmd_volume_raycast's.  Every other seed is left as it is, and the state
+ * stays UPDATE: new frames still have to confirm the prior.  So after the
+ * in-place propagation (rmd_seeds_set_prior_propagation) or
+ * rmd_seeds_propagate_prior, the volume wins where it has a hit and the
+ * splatted or uniform prior stays elsewhere.  A volume never integrated leaves
+ * s as set_reference left it.
+ *
+ * Asynchronous, no host synchronisation: the rays run on s's stream after
+ * everything already enqueued on the volume's stream (e.g. the
+ * rmd_volume_integrate_seeds of the keyframe just left) and after work another
+ * handle enqueued against s; a later integrate, reset or upload of the volume
+ * waits for the rays.  RMD_ERR_INVALID_ARGUMENT: null handle, volume and seeds
+ * on different devices, sigma_sq_frac outside (0, 1].  RMD_ERR_NOT_INITIALISED:
+ * s has no reference or has been updated since it was set. */
+int rmd_volume_prior_seeds(rmd_volume_t *v, rmd_seeds_t *s, float sigma_sq_frac);
+
 /* Test / checkpoint hooks (like rmd_seeds_upload_state): nx * ny * nz floats
  * each, x fastest.  Synchronous. */
 int rmd_volume_download(rmd_volume_t *v, float *host_tsdf, float *host_weight);

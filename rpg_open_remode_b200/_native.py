@@ -84,6 +84,7 @@ _SIGNATURES = {
     "rmd_volume_mesh": (ci, [vp, vp, cs, vp, cs, P(cs), P(cs)]),
     "rmd_volume_mesh_device": (ci, [vp, vp, cs, vp, cs, P(cs), P(cs)]),
     "rmd_volume_raycast": (ci, [vp, ci, ci, cf, cf, cf, cf, vp, vp, cs]),
+    "rmd_volume_prior_seeds": (ci, [vp, vp, cf]),
     "rmd_volume_download": (ci, [vp, vp, vp]),
     "rmd_volume_upload": (ci, [vp, vp, vp]),
     "rmd_volume_enable_intensity": (ci, [vp]),

@@ -381,6 +381,14 @@ class SeedMatrix:
         check(self._L.rmd_seeds_propagate_prior(self._h, src.handle, float(sigma_sq_frac)),
               "SeedMatrix::propagatePriorFrom")
 
+    def priorFromVolume(self, volume: "TsdfVolume", sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC) -> None:
+        """Right after setReferenceImage* (no update since): every pixel whose ray from the new reference pose hits
+        the fused surface of `volume` within [min_depth, max_depth] takes the hit as its depth prior (sigma^2 =
+        sigma_sq_frac * range^2 / 36); all other seeds keep the prior they have (uniform, or splatted by the
+        propagation above).  Ordered on the device after the volume's queued integrations."""
+        check(self._L.rmd_volume_prior_seeds(volume.handle, self._h, float(sigma_sq_frac)),
+              "SeedMatrix::priorFromVolume")
+
     def uploadState(self, field: int, values) -> None:
         dt = np.int32 if field == FIELD_CONVERGENCE else np.float32
         a = np.ascontiguousarray(values, dtype=dt)
@@ -779,6 +787,11 @@ class Depthmap:
         """Each new reference frame takes its depth prior from the converged seeds of the keyframe it replaces
         (SeedMatrix.setPriorPropagation); 0 switches it off (the default of a new Depthmap)."""
         self.seeds_.setPriorPropagation(sigma_sq_frac)
+
+    def priorFromVolume(self, volume: TsdfVolume, sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC) -> None:
+        """After setReferenceImage: the new keyframe's depth prior from the model fused so far
+        (SeedMatrix.priorFromVolume)."""
+        self.seeds_.priorFromVolume(volume, sigma_sq_frac)
 
     def update(self, img_curr, T_curr_world) -> None:
         self.seeds_.update(self._input_image(img_curr), T_curr_world)

@@ -7,7 +7,7 @@
 // the legacy default stream, a pinned upload ring with a copy stream so the
 // H2D transfer of frame k+1 overlaps the kernel of frame k, one fused launch
 // per frame and no device synchronisation inside update().  The TSDF volume's entry points are in volume_api.cu,
-// except rmd_volume_integrate_seeds, which reads the seeds' internals.
+// except rmd_volume_integrate_seeds and rmd_volume_prior_seeds, which read the seeds' internals.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -2098,7 +2098,7 @@ int rmd_image_copy(void *dst, size_t dst_pitch, const void *src, size_t src_pitc
 } // extern "C"
 
 // ============================================================ TSDF volume
-// The volume's entry points are in volume_api.cu; this one reads the seeds' internals and orders the volume's
+// The volume's entry points are in volume_api.cu; these two read the seeds' internals and order the volume's
 // stream against theirs.
 
 extern "C"
@@ -2141,6 +2141,44 @@ int rmd_volume_integrate_seeds(rmd_volume_t *v, rmd_seeds_t *s, const float *dev
   // ... and a later writer of the seeds (update, set_reference, upload_state) waits for the kernel's reads
   RMD_CUDA_TRY(cudaEventRecord(s->ext_ev, v->stream));
   s->ext_pending = true;
+  return 0;
+}
+
+int rmd_volume_prior_seeds(rmd_volume_t *v, rmd_seeds_t *s, float sigma_sq_frac)
+{
+  RMD_REQUIRE(v && s, "rmd_volume_prior_seeds: null handle");
+  RMD_REQUIRE(v->device == s->device, "rmd_volume_prior_seeds: volume and seeds on different devices");
+  RMD_REQUIRE(sigma_sq_frac > 0.0f && sigma_sq_frac <= 1.0f, "rmd_volume_prior_seeds: sigma_sq_frac must be in (0, 1]");
+  if(!s->has_reference || s->frame_index != 0)
+    return fail(RMD_ERR_NOT_INITIALISED,
+                "rmd_volume_prior_seeds: the seeds need a reference frame set since their last update");
+  DeviceGuard guard(s->device);
+  {
+    const int rc = wait_external(s);
+    if(rc) return rc;
+  }
+  // The rays run on the seeds' stream and read the model as the volume's queued work leaves it (e.g. the
+  // integration of the keyframe just left) ...
+  RMD_CUDA_TRY(cudaEventRecord(v->seeds_ev, v->stream));
+  RMD_CUDA_TRY(cudaStreamWaitEvent(s->stream, v->seeds_ev, 0));
+  VolumeRaycastParams P;
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.width = s->width; P.height = s->height;
+  P.cam = s->cam;
+  P.T_world_curr = s->T_world_ref;   // = pose_inverse(pose_from(T_curr_world)), as rmd_volume_raycast computes it
+  VolumePriorSeeds S;
+  memset(&S, 0, sizeof(S));
+  S.seed = s->seed; S.seed_stride = s->seed_stride;
+  S.conv = s->conv; S.conv_stride = (int)(s->conv_pitch / sizeof(int));
+  S.min_depth = s->min_depth; S.max_depth = s->max_depth;
+  S.sigma_sq = sigma_sq_frac * s->sigma_sq_max;   // as prior_apply
+  RMD_CUDA_TRY(launch_volume_prior(P, S, s->stream));
+  s->n_total += 1;
+  // ... and a later writer of the volume (integrate, reset, upload) waits for the rays' reads.  The wait above has
+  // already taken the event's previous record, so recording it again loses nothing.
+  RMD_CUDA_TRY(cudaEventRecord(v->seeds_ev, s->stream));
+  RMD_CUDA_TRY(cudaStreamWaitEvent(v->stream, v->seeds_ev, 0));
   return 0;
 }
 

@@ -443,10 +443,13 @@ __device__ __forceinline__ bool sample_records(const VolumeGrid &g, const float2
   return true;
 }
 
-// The ray of pixel (x, y).  INTENSITY: also the intensity at the hit, from the grid coordinates of org + t dir in the
-// march's form (the plain instance ignores C).
+// The march of the ray of pixel (x, y): the distance to the first zero crossing, 0 where there is none.  INTENSITY:
+// also the intensity at the hit into inten (-1 = none), from the grid coordinates of org + t dir in the march's form
+// (the plain instance ignores C and inten).  The raycast and the volume prior share it, so that the prior's depth is
+// the raycast's, bit for bit.
 template<bool INTENSITY>
-__device__ __forceinline__ void raycast_pixel(const VolumeRaycastParams &P, const VolumeRaycastColour &C, int x, int y)
+__device__ __forceinline__ float raycast_hit(const VolumeRaycastParams &P, const VolumeRaycastColour &C, int x, int y,
+                                             float &inten)
 {
   const VolumeGrid &g = P.g;
   // the ray of back_project (point_cloud.cuh), rotated into the world; it starts at the camera centre
@@ -479,7 +482,7 @@ __device__ __forceinline__ void raycast_pixel(const VolumeRaycastParams &P, cons
     t0 = fmaxf(t0, fminf(ta, tb));
     t1 = fminf(t1, fmaxf(ta, tb));
   }
-  float out = 0.0f, inten = -1.0f;
+  float out = 0.0f;
   if(inside && t0 <= t1)
   {
     // a segment inside the box is at most nx + ny + nz voxels long: the bound only stops a ray whose steps
@@ -513,9 +516,7 @@ __device__ __forceinline__ void raycast_pixel(const VolumeRaycastParams &P, cons
       f_prev = f;
     }
   }
-  P.depth[(size_t)y * P.depth_stride + x] = out;
-  if(INTENSITY)
-    C.intensity[(size_t)y * C.intensity_stride + x] = inten;
+  return out;
 }
 
 // The colour fields are a parameter of their own: past 128 B a parameter is read through a pointer, which slows the
@@ -527,7 +528,29 @@ __global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycast
   const int y = blockIdx.y * blockDim.y + threadIdx.y;
   if(x >= P.width || y >= P.height)
     return;
-  raycast_pixel<INTENSITY>(P, C, x, y);
+  float inten = -1.0f;
+  P.depth[(size_t)y * P.depth_stride + x] = raycast_hit<INTENSITY>(P, C, x, y, inten);
+  if(INTENSITY)
+    C.intensity[(size_t)y * C.intensity_stride + x] = inten;
+}
+
+// One ray per pixel of the seeds' image; a BORDER pixel is not marched.  A hit within [min_depth, max_depth] becomes
+// the seed (d, sigma_sq, 10, 10) in one 16-byte store; every other seed is left as it is.
+__global__ void __launch_bounds__(256) volume_prior_kernel(const VolumeRaycastParams P, const VolumePriorSeeds S)
+{
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const int y = blockIdx.y * blockDim.y + threadIdx.y;
+  if(x >= P.width || y >= P.height)
+    return;
+  if(S.conv[(size_t)y * S.conv_stride + x] == RMD_BORDER)
+    return;
+  const VolumeRaycastColour none = {};
+  float unused;
+  const float d = raycast_hit<false>(P, none, x, y, unused);
+  if(!(d > 0.0f && d >= S.min_depth && d <= S.max_depth))
+    return;
+  // a = b = 10: inlier ratio 0.5, so the seed cannot be CONVERGED before new frames confirm it (as prior_apply_kernel)
+  S.seed[(size_t)y * S.seed_stride + x] = make_float4(d, S.sigma_sq, 10.0f, 10.0f);
 }
 
 } // namespace
@@ -585,6 +608,14 @@ cudaError_t launch_volume_raycast(const VolumeRaycastParams &P, const VolumeRayc
     volume_raycast_kernel<true><<<grid, block, 0, stream>>>(P, C);
   else
     volume_raycast_kernel<false><<<grid, block, 0, stream>>>(P, C);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_prior(const VolumeRaycastParams &P, const VolumePriorSeeds &S, cudaStream_t stream)
+{
+  const dim3 block(32, 8);
+  const dim3 grid((P.width + block.x - 1) / block.x, (P.height + block.y - 1) / block.y);
+  volume_prior_kernel<<<grid, block, 0, stream>>>(P, S);
   return cudaGetLastError();
 }
 

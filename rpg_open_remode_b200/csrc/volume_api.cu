@@ -1,6 +1,6 @@
 // volume_api.cu -- the C-ABI of the TSDF volume (rmd_volume_*, include/rmd_b200.h; DESIGN.md 4.8): the handle,
 // argument checks, scratch and staging buffers, and the host sequencing of the kernels in volume.cu.
-// rmd_volume_integrate_seeds is in c_api.cu, next to the seeds' internals it reads.
+// rmd_volume_integrate_seeds and rmd_volume_prior_seeds are in c_api.cu, next to the seeds' internals they read.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>

@@ -30,9 +30,15 @@ class DepthmapNode:
 
     def __init__(self, depthmap: Depthmap, ref_compl_perc: float = 10.0, max_dist_from_ref: float = 0.5,
                  publish_conv_every_n: int = 10, publisher: Optional[Callable] = None,
-                 volume: Optional[TsdfVolume] = None):
+                 volume: Optional[TsdfVolume] = None, prior_from_volume: float = 0.0):
+        if prior_from_volume and volume is None:
+            raise ValueError("DepthmapNode: prior_from_volume needs a volume")
+        if not 0.0 <= prior_from_volume <= 1.0:
+            raise ValueError("DepthmapNode: prior_from_volume must be in [0, 1] (0 = off)")
         self.depthmap_ = depthmap
         self.volume_ = volume   # when given, every finished keyframe is fused into it (DESIGN.md 4.8)
+        # sigma^2 fraction of the new keyframe's prior raycast from volume_ (0 = off)
+        self.prior_from_volume_ = float(prior_from_volume)
         self.state_ = TAKE_REFERENCE_FRAME                      # src/depthmap_node.cpp:35
         self.ref_compl_perc_ = float(ref_compl_perc)            # :81, default 10.0
         self.max_dist_from_ref_ = float(max_dist_from_ref)      # :82, default 0.5
@@ -48,6 +54,8 @@ class DepthmapNode:
         if self.state_ == TAKE_REFERENCE_FRAME:
             if self.depthmap_.setReferenceImage(img_8uc1, T_curr_world, min_depth, max_depth):
                 self.state_ = UPDATE                                              # :126-135
+                if self.prior_from_volume_:   # the volume holds every keyframe published so far
+                    self.depthmap_.priorFromVolume(self.volume_, self.prior_from_volume_)
         elif self.state_ == UPDATE:
             self.depthmap_.update(img_8uc1, T_curr_world)                         # :142
             perc_conv = self.depthmap_.getConvergedPercentage()                   # :143
@@ -83,13 +91,18 @@ class KeyframeSet:
         self.live: List[bool] = [False] * n
 
     def setReferenceImage(self, slot: int, img, T_curr_world, min_depth: float, max_depth: float,
-                          prior_from: Optional[int] = None, sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC) -> None:
-        """prior_from: another live slot whose converged seeds become the new keyframe's depth prior."""
+                          prior_from: Optional[int] = None, sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC,
+                          prior_volume: Optional[TsdfVolume] = None) -> None:
+        """prior_from: another live slot whose converged seeds become the new keyframe's depth prior.
+        prior_volume: a TSDF volume whose raycast from the new reference pose becomes the prior where it hits (over
+        prior_from's where both give one)."""
         if prior_from is not None and (prior_from == slot or not self.live[prior_from]):
             raise ValueError("KeyframeSet.setReferenceImage: prior_from must be another live slot")
         self.seeds[slot].setReferenceImage(img, T_curr_world, min_depth, max_depth)
         if prior_from is not None:
             self.seeds[slot].propagatePriorFrom(self.seeds[prior_from], sigma_sq_frac)
+        if prior_volume is not None:
+            self.seeds[slot].priorFromVolume(prior_volume, sigma_sq_frac)
         self.live[slot] = True
 
     def retire(self, slot: int) -> None:
