@@ -136,6 +136,31 @@ public:
                            "TsdfVolume: unable to raycast the intensity");
   }
 
+  // One unit normal (nx, ny, nz, 0) per surface point (= mesh vertex), in surfacePoints() order, towards free space;
+  // (0, 0, 0, 0) where the tsdf gradient vanishes.
+  std::vector<float> surfaceNormals()
+  {
+    size_t n = 0;
+    detail::throw_on_error(rmd_volume_surface_normals(handle_, NULL, 0, &n), "TsdfVolume: unable to count points");
+    std::vector<float> out(4 * n);
+    if(n)
+      detail::throw_on_error(rmd_volume_surface_normals(handle_, out.data(), n, &n),
+                             "TsdfVolume: unable to extract the normals");
+    out.resize(4 * n < out.size() ? 4 * n : out.size());
+    return out;
+  }
+
+  // raycast() and the world-frame normal at each hit ((0, 0, 0, 0) = none) into a pitched device image of float4
+  // (normals_pitch a multiple of 16 bytes); asynchronous.
+  void raycastNormals(int width, int height, const PinholeCamera &cam, const SE3<float> &T_curr_world,
+                      float *dev_depth, size_t depth_pitch, float *dev_normals, size_t normals_pitch)
+  {
+    detail::throw_on_error(rmd_volume_raycast_normals(handle_, width, height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                                      T_curr_world.data.data, dev_depth, depth_pitch, dev_normals,
+                                                      normals_pitch),
+                           "TsdfVolume: unable to raycast the normals");
+  }
+
   void downloadIntensity(float *host_intensity, float *host_weight)
   {
     detail::throw_on_error(rmd_volume_download_intensity(handle_, host_intensity, host_weight),

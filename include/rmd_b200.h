@@ -581,6 +581,36 @@ int rmd_volume_raycast_intensity(rmd_volume_t *v, int width, int height, float f
 int rmd_volume_download_intensity(rmd_volume_t *v, float *host_intensity, float *host_weight);
 int rmd_volume_upload_intensity(rmd_volume_t *v, const float *host_intensity, const float *host_weight);
 
+/* Surface normals (DESIGN.md 4.8), on volumes with or without the intensity
+ * channel.  The gradient of a voxel v with tsdf t0 uses the tsdf records
+ * only (unitless, per voxel): along each axis e, a neighbour v +- e is usable
+ * when it lies inside the grid and has weight > 0, and the component is
+ * (t+ - t-) * 0.5 when both are usable, t+ - t0 or t0 - t- when one is, else
+ * 0.  A normal is g / len with len = sqrt((gx^2 + gy^2) + gz^2), (0, 0, 0)
+ * when len is 0 or not finite; it points towards tsdf > 0 (free space, the
+ * cameras), the side the mesh's (b - a) x (c - a) faces.
+ *
+ * One normal (nx, ny, nz, 0) per surface point / mesh vertex, in
+ * rmd_volume_surface_points' order and count/capacity/staging contract: for
+ * the point of voxel a with neighbour b and factor f = t_a / (t_a - t_b), the
+ * gradients of a and b interpolated per component, g_a + f (g_b - g_a), then
+ * normalised.  Device output 16-byte aligned.  Synchronous. */
+int rmd_volume_surface_normals(rmd_volume_t *v, float *host_nxyz0, size_t capacity, size_t *count);
+int rmd_volume_surface_normals_device(rmd_volume_t *v, float *dev_nxyz0, size_t capacity, size_t *count);
+/* rmd_volume_raycast (dev_depth bit-identical) + a world-frame unit normal
+ * per pixel, float4 (nx, ny, nz, 0): at a hit t, the grid coordinates of
+ * org + t dir as the march computes them, the gradients of the 8 corners of
+ * that cell interpolated trilinearly in x, then y, then z, normalised;
+ * (0, 0, 0, 0) when a corner lies outside the grid or has weight 0, and where
+ * there is no hit.  Along a cube edge this field is the vertex normals' linear
+ * interpolation.  dev_normals 16-byte aligned, normals_pitch (bytes) >= 16 *
+ * width and a multiple of 16.  RMD_ERR_INVALID_ARGUMENT: null handle or
+ * pointer, bad size, pitch or alignment.  Asynchronous on the volume's
+ * stream. */
+int rmd_volume_raycast_normals(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                               const float *T_curr_world, float *dev_depth, size_t depth_pitch,
+                               float *dev_normals, size_t normals_pitch);
+
 /* ---------------------------------------------------------- device image */
 
 /* DeviceImage<T>(width,height) = cudaMallocPitch, device_image.cuh:37-50 */

@@ -609,6 +609,13 @@ class TsdfVolume:
         neither of the point's voxels has one.  With a capacity, at most that many."""
         return self._surface(self._L.rmd_volume_surface_intensity, capacity, (), "TsdfVolume::surfaceIntensity")
 
+    def surfaceNormals(self, capacity: "int | None" = None) -> np.ndarray:
+        """float32 [n, 3]: the unit normal of every surface point (and mesh vertex), in surfacePoints() order,
+        towards free space (tsdf > 0); (0, 0, 0) where the tsdf gradient vanishes.  With a capacity, at most that
+        many."""
+        n = self._surface(self._L.rmd_volume_surface_normals, capacity, (4,), "TsdfVolume::surfaceNormals")
+        return np.ascontiguousarray(n[:, :3])
+
     def mesh(self, vertex_capacity: "int | None" = None, triangle_capacity: "int | None" = None):
         """Marching-cubes mesh of the fused surface: (float32 [n, 4] vertices, int32 [m, 3] triangles).  The vertices
         are surfacePoints(), bit for bit; triangles are ordered by cube and face the tsdf > 0 side, (b - a) x (c - a).
@@ -646,6 +653,18 @@ class TsdfVolume:
               "TsdfVolume::raycastIntensity")
         self.sync()
         return img.getDevData(), inten.getDevData()
+
+    def raycastNormals(self, cam: PinholeCamera, T_curr_world, width: int, height: int):
+        """(depth float32 [height, width], normals float32 [height, width, 3]): raycast()'s depth, bit for bit, and
+        the world-frame unit normal of the fused surface at each hit, (0, 0, 0) where there is no hit or no
+        normal."""
+        img, nrm = DeviceImage(width, height, "float32"), DeviceImage(4 * int(width), height, "float32")
+        T = _pose12(T_curr_world)
+        check(self._L.rmd_volume_raycast_normals(self._h, int(width), int(height), cam.fx, cam.fy, cam.cx, cam.cy,
+                                                 T.ctypes.data, img.data, img.pitch, nrm.data, nrm.pitch),
+              "TsdfVolume::raycastNormals")
+        self.sync()
+        return img.getDevData(), np.ascontiguousarray(nrm.getDevData().reshape(int(height), int(width), 4)[..., :3])
 
     def _download_records(self, fn, what: str):
         """The two halves of a record array (fn: rmd_volume_download[_intensity]), float32 of shape (nz, ny, nx)."""
@@ -685,16 +704,24 @@ class TsdfVolume:
         check(self._L.rmd_volume_sync(self._h), "TsdfVolume::sync")
 
 
-def write_ply(path: str, vertices, triangles, intensity=None) -> None:
+def write_ply(path: str, vertices, triangles, intensity=None, normals=None) -> None:
     """Binary little-endian PLY of a mesh such as TsdfVolume.mesh() returns: per vertex float x, y, z and the
-    weight as float `weight`; per face a uchar-counted int list `vertex_indices`.  With `intensity` (one value per
-    vertex in [0, 1], e.g. TsdfVolume.surfaceIntensity()), each vertex also gets uchar red, green, blue =
-    clip(rint(255 i), 0, 255); -1 (no intensity) is written as 0."""
+    weight as float `weight`; per face a uchar-counted int list `vertex_indices`.  With `normals` (one [3] per
+    vertex, e.g. TsdfVolume.surfaceNormals()), each vertex also gets float nx, ny, nz for smooth shading.  With
+    `intensity` (one value per vertex in [0, 1], e.g. TsdfVolume.surfaceIntensity()), each vertex then gets uchar
+    red, green, blue = clip(rint(255 i), 0, 255); -1 (no intensity) is written as 0."""
     v = np.ascontiguousarray(vertices, "<f4").reshape(-1, 4)
     t = np.ascontiguousarray(triangles, "<i4").reshape(-1, 3)
     faces = np.empty(len(t), np.dtype([("n", "u1"), ("i", "<i4", 3)]))
     faces["n"], faces["i"] = 3, t
-    colour = ""
+    fields, values, extra = [("p", "<f4", 4)], [v], ""
+    if normals is not None:
+        n = np.asarray(normals, np.float32)
+        if n.shape != (len(v), 3):
+            raise ValueError("write_ply: one normal (nx, ny, nz) per vertex")
+        fields.append(("n", "<f4", 3))
+        values.append(n)
+        extra += "property float nx\nproperty float ny\nproperty float nz\n"
     if intensity is not None:
         i = np.asarray(intensity, np.float32).reshape(-1)
         if len(i) != len(v):
@@ -702,13 +729,17 @@ def write_ply(path: str, vertices, triangles, intensity=None) -> None:
         with np.errstate(invalid="ignore"):
             g = np.clip(np.rint(np.float32(255) * i), 0, 255)
         g = np.where(np.isfinite(g), g, 0).astype(np.uint8)
-        rec = np.empty(len(v), np.dtype([("p", "<f4", 4), ("c", "u1", 3)]))
-        rec["p"], rec["c"] = v, g[:, None]
+        fields.append(("c", "u1", 3))
+        values.append(np.repeat(g[:, None], 3, 1))
+        extra += "property uchar red\nproperty uchar green\nproperty uchar blue\n"
+    if len(fields) > 1:
+        rec = np.empty(len(v), np.dtype(fields))
+        for (name, *_), val in zip(fields, values):
+            rec[name] = val
         v = rec
-        colour = "property uchar red\nproperty uchar green\nproperty uchar blue\n"
     header = ("ply\nformat binary_little_endian 1.0\n"
               "element vertex %d\nproperty float x\nproperty float y\nproperty float z\nproperty float weight\n"
-              "%selement face %d\nproperty list uchar int vertex_indices\nend_header\n" % (len(v), colour, len(t)))
+              "%selement face %d\nproperty list uchar int vertex_indices\nend_header\n" % (len(v), extra, len(t)))
     with open(path, "wb") as f:
         f.write(header.encode("ascii"))
         f.write(v.tobytes())

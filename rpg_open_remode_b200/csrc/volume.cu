@@ -163,6 +163,55 @@ __device__ __forceinline__ float surface_intensity(const VolumeSurfaceParams &P,
   return ca.y > 0.0f ? ca.x : cb.y > 0.0f ? cb.x : -1.0f;
 }
 
+// ---------------------------------------------------------------------------------------- normals
+// One component of the tsdf gradient of a known voxel (record index n, tsdf t0) along an axis of index step `step`:
+// the neighbours n - step (when dn) and n + step (when up) lie inside the grid and count when their weight is > 0.
+__device__ __forceinline__ float gradient_component(const float2 *vox, size_t n, size_t step, bool dn, bool up,
+                                                    float t0)
+{
+  float2 m = make_float2(0.0f, 0.0f), p = make_float2(0.0f, 0.0f);
+  if(dn) m = __ldg(vox + n - step);
+  if(up) p = __ldg(vox + n + step);
+  const bool um = m.y > 0.0f, up_ok = p.y > 0.0f;
+  if(um && up_ok) return __fmul_rn(__fsub_rn(p.x, m.x), 0.5f);
+  if(up_ok) return __fsub_rn(p.x, t0);
+  if(um) return __fsub_rn(t0, m.x);
+  return 0.0f;
+}
+
+// The tsdf gradient of known voxel (i, j, k) with tsdf t0 (DESIGN.md 4.8): unitless, per voxel, towards tsdf > 0.
+__device__ __forceinline__ float3 voxel_gradient(const VolumeGrid &g, int i, int j, int k, float t0)
+{
+  const size_t sy = (size_t)g.nx, sz = (size_t)g.nx * (size_t)g.ny;
+  const size_t n = (size_t)k * sz + (size_t)j * sy + (size_t)i;
+  return make_float3(gradient_component(g.vox, n, 1, i > 0, i + 1 < g.nx, t0),
+                     gradient_component(g.vox, n, sy, j > 0, j + 1 < g.ny, t0),
+                     gradient_component(g.vox, n, sz, k > 0, k + 1 < g.nz, t0));
+}
+
+// g / |g| with |g| = sqrt((gx^2 + gy^2) + gz^2); (0, 0, 0) when |g| is 0 or not finite.  The fourth component is 0.
+__device__ __forceinline__ float4 unit_normal(float3 v)
+{
+  const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y)), __fmul_rn(v.z, v.z)));
+  if(!(len > 0.0f) || !finite_f(len))
+    return make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  return make_float4(__fdiv_rn(v.x, len), __fdiv_rn(v.y, len), __fdiv_rn(v.z, len), 0.0f);
+}
+
+__device__ __forceinline__ float3 lerp3_rn(float3 a, float3 b, float f)
+{
+  return make_float3(lerp_rn(a.x, b.x, f), lerp_rn(a.y, b.y, f), lerp_rn(a.z, b.z, f));
+}
+
+// Normal of the point of voxel a = (c.i, c.j, c.k) on `axis`: the gradients of a and of its neighbour b, interpolated
+// with the position's factor t_a / (t_a - t_b), then normalised.
+__device__ __forceinline__ float4 surface_normal(const VolumeGrid &g, const SurfaceCell &c, int axis)
+{
+  const float3 ga = voxel_gradient(g, c.i, c.j, c.k, c.a.x);
+  const float3 gb = voxel_gradient(g, c.i + (axis == 0), c.j + (axis == 1), c.k + (axis == 2), c.b[axis].x);
+  return unit_normal(lerp3_rn(ga, gb, __fdiv_rn(c.a.x, __fsub_rn(c.a.x, c.b[axis].x))));
+}
+
 __device__ __forceinline__ unsigned int grid_voxels(const VolumeGrid &g)
 {
   return (unsigned int)g.nx * (unsigned int)g.ny * (unsigned int)g.nz;   // <= 2^31
@@ -289,8 +338,9 @@ __global__ void __launch_bounds__(VOLUME_SCAN_BLOCK) volume_surface_scan_kernel(
 }
 
 // KEYS (the mesh path): also write every point's key 3 * voxel + axis, for all *total points whatever the capacity.
-// INTENSITY: write every point's intensity to P.intensity instead of its position to P.out.
-template<bool KEYS, bool INTENSITY>
+// INTENSITY: write every point's intensity to P.intensity instead of its position to P.out.  NORMALS: write every
+// point's normal to P.normals instead.
+template<bool KEYS, bool INTENSITY, bool NORMALS>
 __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_write_kernel(const VolumeSurfaceParams P)
 {
   __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
@@ -311,6 +361,8 @@ __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_write_kernel
       {
         if(INTENSITY)
           P.intensity[slot] = surface_intensity(P, c, base + r * VOLUME_SURF_BLOCK, axis);
+        else if(NORMALS)
+          P.normals[slot] = surface_normal(P.g, c, axis);
         else
           P.out[slot] = surface_point(P.g, c, axis);
       }
@@ -443,13 +495,45 @@ __device__ __forceinline__ bool sample_records(const VolumeGrid &g, const float2
   return true;
 }
 
+// The normal at grid coordinates (gx, gy, gz): the gradients of the 8 corners of the cell (which read the cell's
+// records and those of its face neighbours), interpolated trilinearly in x, then y, then z per component, then
+// normalised; (0, 0, 0, 0) if a corner lies outside the grid or has weight 0.
+__device__ __forceinline__ float4 sample_normal(const VolumeGrid &g, float gx, float gy, float gz)
+{
+  const float4 none = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  const float x0 = floorf(gx), y0 = floorf(gy), z0 = floorf(gz);
+  const int i0 = (x0 >= 0.0f && x0 < 2.0e9f) ? (int)x0 : -1;
+  const int j0 = (y0 >= 0.0f && y0 < 2.0e9f) ? (int)y0 : -1;
+  const int k0 = (z0 >= 0.0f && z0 < 2.0e9f) ? (int)z0 : -1;
+  if(i0 < 0 || j0 < 0 || k0 < 0 || i0 + 1 >= g.nx || j0 + 1 >= g.ny || k0 + 1 >= g.nz)
+    return none;
+  const size_t plane = (size_t)g.nx * g.ny;
+  const float2 *b = g.vox + ((size_t)k0 * g.ny + j0) * g.nx + i0;
+  const float2 c000 = __ldg(b), c100 = __ldg(b + 1), c010 = __ldg(b + g.nx), c110 = __ldg(b + g.nx + 1);
+  const float2 c001 = __ldg(b + plane), c101 = __ldg(b + plane + 1), c011 = __ldg(b + plane + g.nx),
+               c111 = __ldg(b + plane + g.nx + 1);
+  if(c000.y == 0.0f || c100.y == 0.0f || c010.y == 0.0f || c110.y == 0.0f || c001.y == 0.0f || c101.y == 0.0f ||
+     c011.y == 0.0f || c111.y == 0.0f)
+    return none;
+  const float fx = __fsub_rn(gx, x0), fy = __fsub_rn(gy, y0), fz = __fsub_rn(gz, z0);
+  const float3 c00 = lerp3_rn(voxel_gradient(g, i0, j0, k0, c000.x), voxel_gradient(g, i0 + 1, j0, k0, c100.x), fx);
+  const float3 c10 = lerp3_rn(voxel_gradient(g, i0, j0 + 1, k0, c010.x),
+                              voxel_gradient(g, i0 + 1, j0 + 1, k0, c110.x), fx);
+  const float3 c01 = lerp3_rn(voxel_gradient(g, i0, j0, k0 + 1, c001.x),
+                              voxel_gradient(g, i0 + 1, j0, k0 + 1, c101.x), fx);
+  const float3 c11 = lerp3_rn(voxel_gradient(g, i0, j0 + 1, k0 + 1, c011.x),
+                              voxel_gradient(g, i0 + 1, j0 + 1, k0 + 1, c111.x), fx);
+  return unit_normal(lerp3_rn(lerp3_rn(c00, c10, fy), lerp3_rn(c01, c11, fy), fz));
+}
+
 // The march of the ray of pixel (x, y): the distance to the first zero crossing, 0 where there is none.  INTENSITY:
 // also the intensity at the hit into inten (-1 = none), from the grid coordinates of org + t dir in the march's form
-// (the plain instance ignores C and inten).  The raycast and the volume prior share it, so that the prior's depth is
-// the raycast's, bit for bit.
-template<bool INTENSITY>
+// (the plain instance ignores C and inten).  NORMALS: also the normal at the hit, from the same grid coordinates, into
+// normal (left as it is where there is no hit).  The raycasts and the volume prior share it, so that their depths are
+// the plain raycast's, bit for bit.
+template<bool INTENSITY, bool NORMALS>
 __device__ __forceinline__ float raycast_hit(const VolumeRaycastParams &P, const VolumeRaycastColour &C, int x, int y,
-                                             float &inten)
+                                             float &inten, float4 &normal)
 {
   const VolumeGrid &g = P.g;
   // the ray of back_project (point_cloud.cuh), rotated into the world; it starts at the camera centre
@@ -504,11 +588,16 @@ __device__ __forceinline__ float raycast_hit(const VolumeRaycastParams &P, const
       if(known && prev_known && f_prev > 0.0f && f <= 0.0f)
       {
         out = __fadd_rn(t_prev, __fdiv_rn(__fmul_rn(s, f_prev), __fsub_rn(f_prev, f)));
-        if(INTENSITY &&
-           !sample_records(g, C.col, __fdiv_rn(__fsub_rn(__fadd_rn(org[0], __fmul_rn(out, dir[0])), g.ox), s),
-                           __fdiv_rn(__fsub_rn(__fadd_rn(org[1], __fmul_rn(out, dir[1])), g.oy), s),
-                           __fdiv_rn(__fsub_rn(__fadd_rn(org[2], __fmul_rn(out, dir[2])), g.oz), s), inten))
-          inten = -1.0f;
+        if(INTENSITY || NORMALS)
+        {
+          const float hx = __fdiv_rn(__fsub_rn(__fadd_rn(org[0], __fmul_rn(out, dir[0])), g.ox), s);
+          const float hy = __fdiv_rn(__fsub_rn(__fadd_rn(org[1], __fmul_rn(out, dir[1])), g.oy), s);
+          const float hz = __fdiv_rn(__fsub_rn(__fadd_rn(org[2], __fmul_rn(out, dir[2])), g.oz), s);
+          if(INTENSITY && !sample_records(g, C.col, hx, hy, hz, inten))
+            inten = -1.0f;
+          if(NORMALS)
+            normal = sample_normal(g, hx, hy, hz);
+        }
         break;
       }
       prev_known = known;
@@ -529,9 +618,26 @@ __global__ void __launch_bounds__(256) volume_raycast_kernel(const VolumeRaycast
   if(x >= P.width || y >= P.height)
     return;
   float inten = -1.0f;
-  P.depth[(size_t)y * P.depth_stride + x] = raycast_hit<INTENSITY>(P, C, x, y, inten);
+  float4 unused;
+  P.depth[(size_t)y * P.depth_stride + x] = raycast_hit<INTENSITY, false>(P, C, x, y, inten, unused);
   if(INTENSITY)
     C.intensity[(size_t)y * C.intensity_stride + x] = inten;
+}
+
+// The plain rays plus the normal at each hit, one 16-byte store per pixel; the normal outputs are a parameter of
+// their own, like the colour fields.
+__global__ void __launch_bounds__(256) volume_raycast_normals_kernel(const VolumeRaycastParams P,
+                                                                     const VolumeRaycastNormals N)
+{
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const int y = blockIdx.y * blockDim.y + threadIdx.y;
+  if(x >= P.width || y >= P.height)
+    return;
+  const VolumeRaycastColour none = {};
+  float unused;
+  float4 normal = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  P.depth[(size_t)y * P.depth_stride + x] = raycast_hit<false, true>(P, none, x, y, unused, normal);
+  N.normals[(size_t)y * N.normals_stride + x] = normal;
 }
 
 // One ray per pixel of the seeds' image; a BORDER pixel is not marched.  A hit within [min_depth, max_depth] becomes
@@ -546,7 +652,8 @@ __global__ void __launch_bounds__(256) volume_prior_kernel(const VolumeRaycastPa
     return;
   const VolumeRaycastColour none = {};
   float unused;
-  const float d = raycast_hit<false>(P, none, x, y, unused);
+  float4 unused_normal;
+  const float d = raycast_hit<false, false>(P, none, x, y, unused, unused_normal);
   if(!(d > 0.0f && d >= S.min_depth && d <= S.max_depth))
     return;
   // a = b = 10: inlier ratio 0.5, so the seed cannot be CONVERGED before new frames confirm it (as prior_apply_kernel)
@@ -577,11 +684,13 @@ cudaError_t launch_volume_surface_count(const VolumeSurfaceParams &P, cudaStream
 cudaError_t launch_volume_surface_write(const VolumeSurfaceParams &P, cudaStream_t stream)
 {
   if(P.keys)
-    volume_surface_write_kernel<true, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+    volume_surface_write_kernel<true, false, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   else if(P.intensity)
-    volume_surface_write_kernel<false, true><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+    volume_surface_write_kernel<false, true, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+  else if(P.normals)
+    volume_surface_write_kernel<false, false, true><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   else
-    volume_surface_write_kernel<false, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
+    volume_surface_write_kernel<false, false, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P);
   return cudaGetLastError();
 }
 
@@ -608,6 +717,15 @@ cudaError_t launch_volume_raycast(const VolumeRaycastParams &P, const VolumeRayc
     volume_raycast_kernel<true><<<grid, block, 0, stream>>>(P, C);
   else
     volume_raycast_kernel<false><<<grid, block, 0, stream>>>(P, C);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_raycast_normals(const VolumeRaycastParams &P, const VolumeRaycastNormals &N,
+                                          cudaStream_t stream)
+{
+  const dim3 block(32, 8);
+  const dim3 grid((P.width + block.x - 1) / block.x, (P.height + block.y - 1) / block.y);
+  volume_raycast_normals_kernel<<<grid, block, 0, stream>>>(P, N);
   return cudaGetLastError();
 }
 

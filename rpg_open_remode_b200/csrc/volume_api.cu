@@ -74,11 +74,14 @@ int volume_surface_params(rmd_volume *v, VolumeSurfaceParams &P)
   return 0;
 }
 
+enum SurfaceOutput { SURFACE_POINTS, SURFACE_INTENSITY, SURFACE_NORMALS };
+
 // The surface points' count pass and scan, one host read of the count, then for min(count, capacity) points their
-// write pass: positions (float4), or with intensity every point's intensity (float, same blocks and ranks).  host:
-// staged in v->stage and copied to out.  Synchronous.
-int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, bool host, bool intensity)
+// write pass (same blocks and ranks): positions (float4), intensities (float) or normals (float4).  host: staged in
+// v->stage and copied to out.  Synchronous.
+int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, bool host, SurfaceOutput kind)
 {
+  const bool intensity = kind == SURFACE_INTENSITY;
   VolumeSurfaceParams P;
   int rc = volume_surface_params(v, P);
   if(rc) return rc;
@@ -104,6 +107,8 @@ int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, boo
     P.col = v->col;
     P.intensity = static_cast<float*>(dst);
   }
+  else if(kind == SURFACE_NORMALS)
+    P.normals = static_cast<float4*>(dst);
   else
     P.out = static_cast<float4*>(dst);
   RMD_CUDA_TRY(launch_volume_surface_write(P, v->stream));
@@ -219,6 +224,20 @@ int volume_integrate_depth(const char *what, rmd_volume_t *v, int width, int hei
   return volume_integrate(v, P);
 }
 
+// The rays of a pinhole camera at T_curr_world into the volume, writing their depth to dev_depth.
+VolumeRaycastParams raycast_params(rmd_volume *v, int width, int height, float fx, float fy, float cx, float cy,
+                                   const float *T_curr_world, float *dev_depth, size_t depth_pitch)
+{
+  VolumeRaycastParams P;
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.width = width; P.height = height;
+  P.cam.fx = fx; P.cam.fy = fy; P.cam.cx = cx; P.cam.cy = cy;
+  P.T_world_curr = pose_inverse(pose_from(T_curr_world));
+  P.depth = dev_depth; P.depth_stride = depth_pitch / sizeof(float);
+  return P;
+}
+
 // rmd_volume_raycast[_intensity]: with_intensity also requires and writes the intensity image.
 int volume_raycast(const char *what, rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
                    const float *T_curr_world, float *dev_depth, size_t depth_pitch, bool with_intensity,
@@ -234,13 +253,7 @@ int volume_raycast(const char *what, rmd_volume_t *v, int width, int height, flo
       return no_intensity(what);
   }
   DeviceGuard guard(v->device);
-  VolumeRaycastParams P;
-  memset(&P, 0, sizeof(P));
-  P.g = v->g;
-  P.width = width; P.height = height;
-  P.cam.fx = fx; P.cam.fy = fy; P.cam.cx = cx; P.cam.cy = cy;
-  P.T_world_curr = pose_inverse(pose_from(T_curr_world));
-  P.depth = dev_depth; P.depth_stride = depth_pitch / sizeof(float);
+  const VolumeRaycastParams P = raycast_params(v, width, height, fx, fy, cx, cy, T_curr_world, dev_depth, depth_pitch);
   VolumeRaycastColour C;
   memset(&C, 0, sizeof(C));
   if(with_intensity)
@@ -249,6 +262,26 @@ int volume_raycast(const char *what, rmd_volume_t *v, int width, int height, flo
     C.intensity = dev_intensity; C.intensity_stride = intensity_pitch / sizeof(float);
   }
   RMD_CUDA_TRY(launch_volume_raycast(P, C, v->stream));
+  return 0;
+}
+
+// rmd_volume_raycast_normals: the plain rays and a float4 normal per pixel.
+int volume_raycast_normals(const char *what, rmd_volume_t *v, int width, int height, float fx, float fy, float cx,
+                           float cy, const float *T_curr_world, float *dev_depth, size_t depth_pitch,
+                           float *dev_normals, size_t normals_pitch)
+{
+  VOLUME_REQUIRE(v && T_curr_world && dev_depth && dev_normals, "null argument");
+  VOLUME_REQUIRE(width > 0 && height > 0, "bad image size");
+  VOLUME_REQUIRE(depth_pitch_ok(depth_pitch, width), "bad depth pitch");
+  VOLUME_REQUIRE(normals_pitch >= sizeof(float4) * (size_t)width && normals_pitch % sizeof(float4) == 0,
+                 "bad normals pitch");
+  VOLUME_REQUIRE(((uintptr_t)dev_normals % 16) == 0, "normals must be 16-byte aligned");
+  DeviceGuard guard(v->device);
+  const VolumeRaycastParams P = raycast_params(v, width, height, fx, fy, cx, cy, T_curr_world, dev_depth, depth_pitch);
+  VolumeRaycastNormals N;
+  N.normals = reinterpret_cast<float4*>(dev_normals);
+  N.normals_stride = normals_pitch / sizeof(float4);
+  RMD_CUDA_TRY(launch_volume_raycast_normals(P, N, v->stream));
   return 0;
 }
 
@@ -438,7 +471,7 @@ int rmd_volume_surface_points(rmd_volume_t *v, float *host_xyzw, size_t capacity
 {
   RMD_REQUIRE(v && count && (host_xyzw || capacity == 0), "rmd_volume_surface_points: null argument");
   DeviceGuard guard(v->device);
-  return volume_surface(v, host_xyzw, capacity, count, true, false);
+  return volume_surface(v, host_xyzw, capacity, count, true, SURFACE_POINTS);
 }
 
 int rmd_volume_surface_points_device(rmd_volume_t *v, float *dev_xyzw, size_t capacity, size_t *count)
@@ -446,7 +479,7 @@ int rmd_volume_surface_points_device(rmd_volume_t *v, float *dev_xyzw, size_t ca
   RMD_REQUIRE(v && count && (dev_xyzw || capacity == 0), "rmd_volume_surface_points_device: null argument");
   RMD_REQUIRE(((uintptr_t)dev_xyzw % 16) == 0, "rmd_volume_surface_points_device: output must be 16-byte aligned");
   DeviceGuard guard(v->device);
-  return volume_surface(v, dev_xyzw, capacity, count, false, false);
+  return volume_surface(v, dev_xyzw, capacity, count, false, SURFACE_POINTS);
 }
 
 int rmd_volume_surface_intensity(rmd_volume_t *v, float *host_intensity, size_t capacity, size_t *count)
@@ -455,7 +488,7 @@ int rmd_volume_surface_intensity(rmd_volume_t *v, float *host_intensity, size_t 
   if(!v->col)
     return no_intensity("rmd_volume_surface_intensity");
   DeviceGuard guard(v->device);
-  return volume_surface(v, host_intensity, capacity, count, true, true);
+  return volume_surface(v, host_intensity, capacity, count, true, SURFACE_INTENSITY);
 }
 
 int rmd_volume_surface_intensity_device(rmd_volume_t *v, float *dev_intensity, size_t capacity, size_t *count)
@@ -465,7 +498,22 @@ int rmd_volume_surface_intensity_device(rmd_volume_t *v, float *dev_intensity, s
   if(!v->col)
     return no_intensity("rmd_volume_surface_intensity_device");
   DeviceGuard guard(v->device);
-  return volume_surface(v, dev_intensity, capacity, count, false, true);
+  return volume_surface(v, dev_intensity, capacity, count, false, SURFACE_INTENSITY);
+}
+
+int rmd_volume_surface_normals(rmd_volume_t *v, float *host_nxyz0, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (host_nxyz0 || capacity == 0), "rmd_volume_surface_normals: null argument");
+  DeviceGuard guard(v->device);
+  return volume_surface(v, host_nxyz0, capacity, count, true, SURFACE_NORMALS);
+}
+
+int rmd_volume_surface_normals_device(rmd_volume_t *v, float *dev_nxyz0, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (dev_nxyz0 || capacity == 0), "rmd_volume_surface_normals_device: null argument");
+  RMD_REQUIRE(((uintptr_t)dev_nxyz0 % 16) == 0, "rmd_volume_surface_normals_device: output must be 16-byte aligned");
+  DeviceGuard guard(v->device);
+  return volume_surface(v, dev_nxyz0, capacity, count, false, SURFACE_NORMALS);
 }
 
 int rmd_volume_mesh(rmd_volume_t *v, float *host_xyzw, size_t vertex_capacity, int32_t *host_tri,
@@ -503,6 +551,14 @@ int rmd_volume_raycast_intensity(rmd_volume_t *v, int width, int height, float f
 {
   return volume_raycast("rmd_volume_raycast_intensity", v, width, height, fx, fy, cx, cy, T_curr_world, dev_depth,
                         depth_pitch, true, dev_intensity, intensity_pitch);
+}
+
+int rmd_volume_raycast_normals(rmd_volume_t *v, int width, int height, float fx, float fy, float cx, float cy,
+                               const float *T_curr_world, float *dev_depth, size_t depth_pitch,
+                               float *dev_normals, size_t normals_pitch)
+{
+  return volume_raycast_normals("rmd_volume_raycast_normals", v, width, height, fx, fy, cx, cy, T_curr_world,
+                                dev_depth, depth_pitch, dev_normals, normals_pitch);
 }
 
 int rmd_volume_download(rmd_volume_t *v, float *host_tsdf, float *host_weight)

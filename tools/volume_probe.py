@@ -1,7 +1,8 @@
 """Device time of the TSDF volume's operations (DESIGN.md 4.8, 6) on bench.py's c2 scene (VGA): integration of one
 keyframe's depth and state map into a 256^3 and a 512^3 grid over the scene, surface-point extraction, the
 triangle mesh (rmd_volume_mesh_device, vertices and triangles) and a VGA raycast, and the intensity channel's
-variants of integration (the frame's image fused too), surface extraction and raycast next to the plain ones.  Each time is the median of REPEATS runs after WARMUP, measured with CUDA events on the volume's stream.
+variants of integration (the frame's image fused too), surface extraction and raycast next to the plain ones, and the
+surface normals and the raycast with normals next to the surface points and the plain raycast.  Each time is the median of REPEATS runs after WARMUP, measured with CUDA events on the volume's stream.
 The achieved bandwidth of an integration counts 16 B per updated voxel (record read + write) and 8 B per pixel
 (depth + state) over its kernel time, against the 3.35 TB/s of the H100 SXM data sheet.  Prints one JSON line with
 the GPU's name and power limit.  GPU box only."""
@@ -69,6 +70,7 @@ def main():
     image = rmd.DeviceImage(W, H, "float32")
     image.setDevData(fr.image)
     out_i = rmd.DeviceImage(W, H, "float32")
+    out_n = rmd.DeviceImage(4 * W, H, "float32")            # float4 normals
     T = np.ascontiguousarray(fr.T_cam_world.reshape(12))
     c = ctypes.c_float
     stream = torch.cuda.Stream()
@@ -106,6 +108,11 @@ def main():
             _native.check(L.rmd_volume_surface_intensity_device(v.handle, points.data, 4 * n * n, ctypes.byref(count)))
 
         ms_pts_i, runs_pts_i = timed(stream, torch, extract_intensity)
+
+        def extract_normals():
+            _native.check(L.rmd_volume_surface_normals_device(v.handle, points.data, 4 * n * n, ctypes.byref(count)))
+
+        ms_pts_n, runs_pts_n = timed(stream, torch, extract_normals)
         n_tri = ctypes.c_size_t()
         tris = rmd.DeviceImage(3 * 8 * n * n, 1, "int32")         # room for 8 n^2 triangles
 
@@ -127,6 +134,12 @@ def main():
                                                          T.ctypes.data, out.data, out.pitch, out_i.data, out_i.pitch))
 
         ms_ray_i, runs_ray_i = timed(stream, torch, raycast_intensity)
+
+        def raycast_normals():
+            _native.check(L.rmd_volume_raycast_normals(v.handle, W, H, c(cam.fx), c(cam.fy), c(cam.cx), c(cam.cy),
+                                                       T.ctypes.data, out.data, out.pitch, out_n.data, out_n.pitch))
+
+        ms_ray_n, runs_ray_n = timed(stream, torch, raycast_normals)
         v.sync()
         hit = int((out.getDevData() > 0).sum())
         algo_bytes = 16 * updated + 8 * W * H
@@ -147,7 +160,11 @@ def main():
             "surface_intensity_ms": ms_pts_i, "surface_intensity_ms_runs": runs_pts_i,
             "surface_intensity_over_points": ms_pts_i / ms_pts,
             "raycast_intensity_vga_ms": ms_ray_i, "raycast_intensity_vga_ms_runs": runs_ray_i,
-            "raycast_intensity_over_plain": ms_ray_i / ms_ray}
+            "raycast_intensity_over_plain": ms_ray_i / ms_ray,
+            "surface_normals_ms": ms_pts_n, "surface_normals_ms_runs": runs_pts_n,
+            "surface_normals_over_points": ms_pts_n / ms_pts,
+            "raycast_normals_vga_ms": ms_ray_n, "raycast_normals_vga_ms_runs": runs_ray_n,
+            "raycast_normals_over_plain": ms_ray_n / ms_ray}
         del v
     try:
         q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
