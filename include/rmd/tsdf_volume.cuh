@@ -161,6 +161,21 @@ public:
                            "TsdfVolume: unable to raycast the normals");
   }
 
+  // Moving volume: voxel (i, j, k) then holds what (i + dx, j + dy, k + dz) held (unknown outside the grid), and the
+  // origin moves by d * voxel_size.  Asynchronous on the volume's stream; the first shift that moves records doubles
+  // the record memory.  Take the spill (below) first.
+  void shift(int dx, int dy, int dz)
+  {
+    const int d[3] = {dx, dy, dz};
+    detail::throw_on_error(rmd_volume_shift(handle_, d), "TsdfVolume: unable to shift");
+  }
+
+  // The points a shift by d would drop, as the subsequence of surfacePoints() / surfaceIntensity() / surfaceNormals()
+  // in their order; call before shift(d).
+  std::vector<float> spillPoints(const int d[3]) { return spill(rmd_volume_spill_points, d, 4); }
+  std::vector<float> spillIntensity(const int d[3]) { return spill(rmd_volume_spill_intensity, d, 1); }
+  std::vector<float> spillNormals(const int d[3]) { return spill(rmd_volume_spill_normals, d, 4); }
+
   void downloadIntensity(float *host_intensity, float *host_weight)
   {
     detail::throw_on_error(rmd_volume_download_intensity(handle_, host_intensity, host_weight),
@@ -192,6 +207,18 @@ public:
 private:
   TsdfVolume(const TsdfVolume &);
   TsdfVolume &operator=(const TsdfVolume &);
+
+  typedef int (*SpillFn)(rmd_volume_t *, const int *, float *, size_t, size_t *);
+  std::vector<float> spill(SpillFn fn, const int d[3], size_t floats_per_point)
+  {
+    size_t n = 0;
+    detail::throw_on_error(fn(handle_, d, NULL, 0, &n), "TsdfVolume: unable to count the spill");
+    std::vector<float> out(floats_per_point * n);
+    if(n)
+      detail::throw_on_error(fn(handle_, d, out.data(), n, &n), "TsdfVolume: unable to extract the spill");
+    out.resize(floats_per_point * n < out.size() ? floats_per_point * n : out.size());
+    return out;
+  }
 
   rmd_volume_t *handle_;
 };

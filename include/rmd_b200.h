@@ -611,6 +611,46 @@ int rmd_volume_raycast_normals(rmd_volume_t *v, int width, int height, float fx,
                                const float *T_curr_world, float *dev_depth, size_t depth_pitch,
                                float *dev_normals, size_t normals_pitch);
 
+/* Moving volume (DESIGN.md 4.8): the grid keeps its size and follows the
+ * camera by whole voxels, handing the surface that leaves it to the caller.
+ *
+ * rmd_volume_shift: afterwards voxel (i, j, k) holds what voxel
+ * (i + dx, j + dy, k + dz) held before, or (0, 0) (unknown) where that voxel
+ * lies outside the grid; the intensity channel moves the same way.  The
+ * volume keeps the origin o0 it was created with and the total offset D
+ * (64-bit): the origin is then o0 + (float)D * voxel_size per axis, rounded
+ * once per operation, so it depends only on the total and never accumulates
+ * rounding.  rmd_volume_size reports it.  d = (0, 0, 0) does nothing; when
+ * |d| >= the dimension on any axis the grid is reset and the origin moves.
+ * Otherwise a kernel gathers the records into a second array that is then
+ * swapped in: a volume that has shifted keeps 2x its record memory (the
+ * second arrays are allocated by the first shift that moves records and
+ * freed by rmd_volume_destroy); one never shifted allocates nothing.
+ * Asynchronous on the volume's stream: later work on it sees the shifted
+ * grid, and work already enqueued keeps reading the records it was launched
+ * with (the rays of rmd_volume_prior_seeds included: the volume's stream
+ * waits for them, so the next shift cannot overwrite what they read).
+ * download, upload and reset act on the current grid.
+ * RMD_ERR_INVALID_ARGUMENT: null handle or pointer, a total offset that
+ * overflows 64 bits or an origin that would not be finite; the volume is then
+ * unchanged. */
+int rmd_volume_shift(rmd_volume_t *v, const int d[3]);
+/* The spill of a shift by d, called BEFORE rmd_volume_shift(v, d): the shift
+ * keeps the box K = [max(0, d), min(n, n + d)) per axis (pre-shift indices),
+ * and a surface point of voxel a and its neighbour b = a + e_axis spills when
+ * a or b lies outside K.  Every point of the current grid either spills or is
+ * a point of the shifted grid.  Each call returns the subsequence of
+ * rmd_volume_surface_points / _intensity / _normals of the current grid made
+ * of the points that spill, in that order and bit for bit, with the same
+ * count / capacity / staging contract (host output).  Synchronous.
+ * RMD_ERR_INVALID_ARGUMENT: null handle, d or count, null buffer with
+ * capacity > 0.  The intensity variant returns RMD_ERR_NOT_INITIALISED on a
+ * volume without the channel. */
+int rmd_volume_spill_points(rmd_volume_t *v, const int d[3], float *host_xyzw, size_t capacity, size_t *count);
+int rmd_volume_spill_intensity(rmd_volume_t *v, const int d[3], float *host_intensity, size_t capacity,
+                               size_t *count);
+int rmd_volume_spill_normals(rmd_volume_t *v, const int d[3], float *host_nxyz0, size_t capacity, size_t *count);
+
 /* ---------------------------------------------------------- device image */
 
 /* DeviceImage<T>(width,height) = cudaMallocPitch, device_image.cuh:37-50 */

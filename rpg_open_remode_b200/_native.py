@@ -97,6 +97,10 @@ _SIGNATURES = {
     "rmd_volume_surface_normals": (ci, [vp, vp, cs, P(cs)]),
     "rmd_volume_surface_normals_device": (ci, [vp, vp, cs, P(cs)]),
     "rmd_volume_raycast_normals": (ci, [vp, ci, ci, cf, cf, cf, cf, vp, vp, cs, vp, cs]),
+    "rmd_volume_shift": (ci, [vp, vp]),
+    "rmd_volume_spill_points": (ci, [vp, vp, vp, cs, P(cs)]),
+    "rmd_volume_spill_intensity": (ci, [vp, vp, vp, cs, P(cs)]),
+    "rmd_volume_spill_normals": (ci, [vp, vp, vp, cs, P(cs)]),
     "rmd_reduce_sum_f32":(ci, [vp, cs, cs, cs, P(cf)]),
     "rmd_reduce_sum_i32": (ci, [vp, cs, cs, cs, P(ctypes.c_int32)]),
     "rmd_reduce_count_eq_i32": (ci, [vp, cs, cs, cs, ctypes.c_int32, P(cs)]),

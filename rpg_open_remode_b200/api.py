@@ -666,6 +666,43 @@ class TsdfVolume:
         self.sync()
         return img.getDevData(), np.ascontiguousarray(nrm.getDevData().reshape(int(height), int(width), 4)[..., :3])
 
+    def shift(self, d) -> None:
+        """Move the grid by whole voxels d = (dx, dy, dz): voxel (i, j, k) then holds what voxel (i + dx, j + dy,
+        k + dz) held, unknown where that lies outside the grid, and the origin moves by d * voxel_size (from the
+        creation origin and the total offset, so it never accumulates rounding).  Asynchronous on the volume's
+        stream.  Take the surface that leaves the grid with spillPoints(d) etc. first."""
+        a = self._offset(d)
+        check(self._L.rmd_volume_shift(self._h, a.ctypes.data), "TsdfVolume::shift")
+        o = np.empty(3, _f32)
+        check(self._L.rmd_volume_size(self._h, None, None, None, None, o.ctypes.data), "TsdfVolume::shift")
+        self.origin = o
+
+    @staticmethod
+    def _offset(d) -> np.ndarray:
+        a = np.asarray(d)
+        if a.shape != (3,) or not np.all(a == np.round(a)) or np.any(np.abs(a.astype(np.float64)) > 2**31 - 1):
+            raise ValueError("TsdfVolume: d must be three whole voxel counts")
+        return np.ascontiguousarray(a.astype(np.int32))
+
+    def _spill(self, fn, d, capacity, shape, what: str) -> np.ndarray:
+        a = self._offset(d)
+        return self._surface(lambda h, out, cap, n: fn(h, a.ctypes.data, out, cap, n), capacity, shape, what)
+
+    def spillPoints(self, d, capacity: "int | None" = None) -> np.ndarray:
+        """The surface points a shift by d would drop (call it before shift(d)): the subsequence of surfacePoints()
+        whose voxel or neighbour leaves the grid, in that order and bit for bit.  With a capacity, at most that
+        many."""
+        return self._spill(self._L.rmd_volume_spill_points, d, capacity, (4,), "TsdfVolume::spillPoints")
+
+    def spillIntensity(self, d, capacity: "int | None" = None) -> np.ndarray:
+        """surfaceIntensity() of the points spillPoints(d) returns, in its order."""
+        return self._spill(self._L.rmd_volume_spill_intensity, d, capacity, (), "TsdfVolume::spillIntensity")
+
+    def spillNormals(self, d, capacity: "int | None" = None) -> np.ndarray:
+        """float32 [n, 3]: surfaceNormals() of the points spillPoints(d) returns, in its order."""
+        n = self._spill(self._L.rmd_volume_spill_normals, d, capacity, (4,), "TsdfVolume::spillNormals")
+        return np.ascontiguousarray(n[:, :3])
+
     def _download_records(self, fn, what: str):
         """The two halves of a record array (fn: rmd_volume_download[_intensity]), float32 of shape (nz, ny, nx)."""
         nx, ny, nz = self.dims

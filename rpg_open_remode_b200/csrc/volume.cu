@@ -337,6 +337,31 @@ __global__ void __launch_bounds__(VOLUME_SCAN_BLOCK) volume_surface_scan_kernel(
     P.total[0] = carry;
 }
 
+// The points of cell c that spill from the kept box K: bit a stays set unless both voxel a and its neighbour on axis a
+// lie inside K (b differs from a only on that axis, and b >= a >= lo there).
+__device__ __forceinline__ unsigned int spill_mask(const VolumeSpillBox &K, const SurfaceCell &c)
+{
+  if(!c.mask)
+    return 0u;
+  const int p[3] = {c.i, c.j, c.k};
+  bool a_in = true;
+#pragma unroll
+  for(int a = 0; a < 3; ++a)
+    a_in = a_in && p[a] >= K.lo[a] && p[a] < K.hi[a];
+  unsigned int kept = 0u;
+#pragma unroll
+  for(int a = 0; a < 3; ++a)
+    kept |= (a_in && p[a] + 1 < K.hi[a]) ? (1u << a) : 0u;
+  return c.mask & ~kept;
+}
+
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_spill_count_kernel(const VolumeSurfaceParams P,
+                                                                               const VolumeSpillBox K)
+{
+  const unsigned int n_vox = grid_voxels(P.g);
+  count_block(P.b, [&](unsigned int n) { return (unsigned int)__popc(spill_mask(K, surface_cell(P.g, n, n_vox))); });
+}
+
 // KEYS (the mesh path): also write every point's key 3 * voxel + axis, for all *total points whatever the capacity.
 // INTENSITY: write every point's intensity to P.intensity instead of its position to P.out.  NORMALS: write every
 // point's normal to P.normals instead.
@@ -373,6 +398,72 @@ __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_surface_write_kernel
     rank += all;
     __syncthreads();   // warp_off is reused by the next round
   }
+}
+
+// volume_surface_write_kernel without keys, on the points that spill from K: the same blocks, rounds and ranks over
+// the spill counts, so that the spill comes out in the surface points' order.  (The surface kernel's body is kept as
+// it is rather than shared: inlining it into a common function reorders operands in its SASS.)
+template<bool INTENSITY, bool NORMALS>
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_spill_write_kernel(const VolumeSurfaceParams P,
+                                                                               const VolumeSpillBox K)
+{
+  __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
+  const unsigned int n_vox = grid_voxels(P.g);
+  const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
+  unsigned long long rank = P.b.block_offsets[blockIdx.x];
+  for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
+  {
+    SurfaceCell c = surface_cell(P.g, base + r * VOLUME_SURF_BLOCK, n_vox);
+    c.mask = spill_mask(K, c);
+    unsigned int all;
+    unsigned long long slot = round_slot(rank, __popc(c.mask), warp_off, all);
+#pragma unroll
+    for(int axis = 0; axis < 3; ++axis)
+    {
+      if(!(c.mask & (1u << axis)) || slot >= P.capacity)
+        continue;
+      if(INTENSITY)
+        P.intensity[slot] = surface_intensity(P, c, base + r * VOLUME_SURF_BLOCK, axis);
+      else if(NORMALS)
+        P.normals[slot] = surface_normal(P.g, c, axis);
+      else
+        P.out[slot] = surface_point(P.g, c, axis);
+      ++slot;
+    }
+    rank += all;
+    __syncthreads();   // warp_off is reused by the next round
+  }
+}
+
+// ------------------------------------------------------------------------------------------------- shift
+// One thread per destination voxel, x fastest: a gather, so that both the loads of a warp (one source row) and its
+// stores are contiguous.
+template<bool INTENSITY>
+__global__ void __launch_bounds__(256) volume_shift_kernel(const VolumeShiftParams P)
+{
+  const VolumeGrid &g = P.g;
+  const unsigned int plane = (unsigned int)g.nx * (unsigned int)g.ny;
+  const unsigned int n = blockIdx.x * blockDim.x + threadIdx.x;   // < 2^31 voxels: fits
+  if(n >= plane * (unsigned int)g.nz)
+    return;
+  const int k = (int)(n / plane);
+  const unsigned int rem = n - (unsigned int)k * plane;
+  const int j = (int)(rem / (unsigned int)g.nx);
+  const int i = (int)(rem - (unsigned int)j * (unsigned int)g.nx);
+  const int si = i + P.dx, sj = j + P.dy, sk = k + P.dz;   // |d| < n: no overflow
+  float2 r = make_float2(0.0f, 0.0f), c = make_float2(0.0f, 0.0f);
+  if((unsigned int)si < (unsigned int)g.nx && (unsigned int)sj < (unsigned int)g.ny &&
+     (unsigned int)sk < (unsigned int)g.nz)
+  {
+    const size_t src = ((size_t)sk * g.ny + sj) * g.nx + si;
+    r = __ldg(g.vox + src);
+    if(INTENSITY)
+      c = __ldg(P.col + src);
+  }
+  const size_t lin = ((size_t)k * g.ny + j) * g.nx + i;
+  P.out[lin] = r;
+  if(INTENSITY)
+    P.col_out[lin] = c;
 }
 
 // --------------------------------------------------------------------------------------------------- mesh
@@ -734,6 +825,36 @@ cudaError_t launch_volume_prior(const VolumeRaycastParams &P, const VolumePriorS
   const dim3 block(32, 8);
   const dim3 grid((P.width + block.x - 1) / block.x, (P.height + block.y - 1) / block.y);
   volume_prior_kernel<<<grid, block, 0, stream>>>(P, S);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_shift(const VolumeShiftParams &P, cudaStream_t stream)
+{
+  const unsigned int n = (unsigned int)P.g.nx * (unsigned int)P.g.ny * (unsigned int)P.g.nz;
+  if(P.col)
+    volume_shift_kernel<true><<<(n + 255u) / 256u, 256, 0, stream>>>(P);
+  else
+    volume_shift_kernel<false><<<(n + 255u) / 256u, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_spill_count(const VolumeSurfaceParams &P, const VolumeSpillBox &K, cudaStream_t stream)
+{
+  volume_spill_count_kernel<<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  cudaError_t err = cudaGetLastError();
+  if(err != cudaSuccess) return err;
+  volume_surface_scan_kernel<<<1, VOLUME_SCAN_BLOCK, 0, stream>>>(P.b);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_spill_write(const VolumeSurfaceParams &P, const VolumeSpillBox &K, cudaStream_t stream)
+{
+  if(P.intensity)
+    volume_spill_write_kernel<true, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  else if(P.normals)
+    volume_spill_write_kernel<false, true><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  else
+    volume_spill_write_kernel<false, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
   return cudaGetLastError();
 }
 

@@ -77,15 +77,19 @@ int volume_surface_params(rmd_volume *v, VolumeSurfaceParams &P)
 enum SurfaceOutput { SURFACE_POINTS, SURFACE_INTENSITY, SURFACE_NORMALS };
 
 // The surface points' count pass and scan, one host read of the count, then for min(count, capacity) points their
-// write pass (same blocks and ranks): positions (float4), intensities (float) or normals (float4).  host: staged in
-// v->stage and copied to out.  Synchronous.
-int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, bool host, SurfaceOutput kind)
+// write pass (same blocks and ranks): positions (float4), intensities (float) or normals (float4).  With a spill box,
+// only the points that spill from it.  host: staged in v->stage and copied to out.  Synchronous.
+int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, bool host, SurfaceOutput kind,
+                   const VolumeSpillBox *spill = NULL)
 {
   const bool intensity = kind == SURFACE_INTENSITY;
   VolumeSurfaceParams P;
   int rc = volume_surface_params(v, P);
   if(rc) return rc;
-  RMD_CUDA_TRY(launch_volume_surface_count(P, v->stream));
+  if(spill)
+    RMD_CUDA_TRY(launch_volume_spill_count(P, *spill, v->stream));
+  else
+    RMD_CUDA_TRY(launch_volume_surface_count(P, v->stream));
   unsigned long long total = 0;
   RMD_CUDA_TRY(cudaMemcpyAsync(&total, v->surf_total, sizeof(total), cudaMemcpyDeviceToHost, v->stream));
   RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
@@ -111,7 +115,10 @@ int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, boo
     P.normals = static_cast<float4*>(dst);
   else
     P.out = static_cast<float4*>(dst);
-  RMD_CUDA_TRY(launch_volume_surface_write(P, v->stream));
+  if(spill)
+    RMD_CUDA_TRY(launch_volume_spill_write(P, *spill, v->stream));
+  else
+    RMD_CUDA_TRY(launch_volume_surface_write(P, v->stream));
   if(host)
     RMD_CUDA_TRY(cudaMemcpyAsync(out, v->stage, bytes, cudaMemcpyDeviceToHost, v->stream));
   RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
@@ -328,6 +335,39 @@ int volume_upload_records(rmd_volume *v, float2 *records, const float *a, const 
   return 0;
 }
 
+// The box a shift by d keeps (VolumeSpillBox), from d clamped to [-n, n]: the same box, without overflow.
+VolumeSpillBox spill_box(const rmd_volume *v, const int d[3])
+{
+  const int n[3] = {v->g.nx, v->g.ny, v->g.nz};
+  VolumeSpillBox K;
+  for(int a = 0; a < 3; ++a)
+  {
+    const int c = d[a] < -n[a] ? -n[a] : d[a] > n[a] ? n[a] : d[a];
+    K.lo[a] = c > 0 ? c : 0;
+    K.hi[a] = c < 0 ? n[a] + c : n[a];
+  }
+  return K;
+}
+
+// rmd_volume_spill_*: the points of the current grid that a shift by d would drop.
+int volume_spill(const char *what, rmd_volume_t *v, const int d[3], void *host_out, size_t capacity, size_t *count,
+                 SurfaceOutput kind)
+{
+  VOLUME_REQUIRE(v && d && count && (host_out || capacity == 0), "null argument");
+  if(kind == SURFACE_INTENSITY && !v->col)
+    return no_intensity(what);
+  DeviceGuard guard(v->device);
+  const VolumeSpillBox K = spill_box(v, d);
+  return volume_surface(v, host_out, capacity, count, true, kind, &K);
+}
+
+// origin + (float)D * s, one rounding per operation as the kernels' voxel_coord (volatile: no contraction)
+float shifted_origin(float origin, long long D, float s)
+{
+  volatile float step = (float)D * s;
+  return origin + step;
+}
+
 } // namespace
 
 extern "C"
@@ -356,6 +396,7 @@ int rmd_volume_create(int nx, int ny, int nz, float voxel_size, const float orig
   v->g.nx = nx; v->g.ny = ny; v->g.nz = nz;
   v->g.voxel = voxel_size;
   v->g.ox = origin[0]; v->g.oy = origin[1]; v->g.oz = origin[2];
+  v->o0[0] = origin[0]; v->o0[1] = origin[1]; v->o0[2] = origin[2];
   v->n_vox = (size_t)(plane * (uint64_t)nz);
   v->trunc = truncation; v->max_weight = max_weight;
   cudaError_t err = cudaStreamCreateWithFlags(&v->own_stream, cudaStreamNonBlocking);
@@ -384,6 +425,7 @@ int rmd_volume_destroy(rmd_volume_t *v)
   cudaFree(v->surf_offsets); cudaFree(v->surf_total); cudaFree(v->stage);
   cudaFree(v->tri_offsets); cudaFree(v->tri_total); cudaFree(v->keys); cudaFree(v->tri_stage);
   cudaFree(v->col);
+  cudaFree(v->vox_alt); cudaFree(v->col_alt);
   cudaGetLastError();
   delete v;
   return 0;
@@ -425,6 +467,74 @@ int rmd_volume_size(rmd_volume_t *v, int *nx, int *ny, int *nz, float *voxel_siz
   if(voxel_size) *voxel_size = v->g.voxel;
   if(origin) { origin[0] = v->g.ox; origin[1] = v->g.oy; origin[2] = v->g.oz; }
   return 0;
+}
+
+int rmd_volume_shift(rmd_volume_t *v, const int d[3])
+{
+  RMD_REQUIRE(v && d, "rmd_volume_shift: null argument");
+  if(!d[0] && !d[1] && !d[2])
+    return 0;
+  const int n[3] = {v->g.nx, v->g.ny, v->g.nz};
+  long long D[3];
+  float o[3];
+  bool gather = true;
+  for(int a = 0; a < 3; ++a)
+  {
+    RMD_REQUIRE(!__builtin_add_overflow(v->D[a], (long long)d[a], &D[a]), "rmd_volume_shift: the total offset overflows");
+    o[a] = shifted_origin(v->o0[a], D[a], v->g.voxel);
+    RMD_REQUIRE(isfinite(o[a]), "rmd_volume_shift: the origin would not be finite");
+    gather = gather && (d[a] < 0 ? -(long long)d[a] : (long long)d[a]) < n[a];
+  }
+  DeviceGuard guard(v->device);
+  if(!gather)   // nothing stays in the grid
+  {
+    RMD_CUDA_TRY(cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->stream));
+    if(v->col)
+      RMD_CUDA_TRY(cudaMemsetAsync(v->col, 0, sizeof(float2) * v->n_vox, v->stream));
+  }
+  else
+  {
+    if(!v->vox_alt)
+      RMD_CUDA_TRY(cudaMalloc(&v->vox_alt, sizeof(float2) * v->n_vox));
+    if(v->col && !v->col_alt)
+      RMD_CUDA_TRY(cudaMalloc(&v->col_alt, sizeof(float2) * v->n_vox));
+    VolumeShiftParams P;
+    memset(&P, 0, sizeof(P));
+    P.g = v->g;
+    P.out = v->vox_alt;
+    if(v->col)
+    {
+      P.col = v->col; P.col_out = v->col_alt;
+    }
+    P.dx = d[0]; P.dy = d[1]; P.dz = d[2];
+    RMD_CUDA_TRY(launch_volume_shift(P, v->stream));
+    // Later work on the stream reads the new arrays.  The next shift writes the old ones, ordered after everything
+    // already on the stream -- including the wait of rmd_volume_prior_seeds for its rays.
+    float2 *t = v->g.vox; v->g.vox = v->vox_alt; v->vox_alt = t;
+    if(v->col)
+    {
+      t = v->col; v->col = v->col_alt; v->col_alt = t;
+    }
+  }
+  for(int a = 0; a < 3; ++a)
+    v->D[a] = D[a];
+  v->g.ox = o[0]; v->g.oy = o[1]; v->g.oz = o[2];
+  return 0;
+}
+
+int rmd_volume_spill_points(rmd_volume_t *v, const int d[3], float *host_xyzw, size_t capacity, size_t *count)
+{
+  return volume_spill("rmd_volume_spill_points", v, d, host_xyzw, capacity, count, SURFACE_POINTS);
+}
+
+int rmd_volume_spill_intensity(rmd_volume_t *v, const int d[3], float *host_intensity, size_t capacity, size_t *count)
+{
+  return volume_spill("rmd_volume_spill_intensity", v, d, host_intensity, capacity, count, SURFACE_INTENSITY);
+}
+
+int rmd_volume_spill_normals(rmd_volume_t *v, const int d[3], float *host_nxyz0, size_t capacity, size_t *count)
+{
+  return volume_spill("rmd_volume_spill_normals", v, d, host_nxyz0, capacity, count, SURFACE_NORMALS);
 }
 
 int rmd_volume_enable_intensity(rmd_volume_t *v)

@@ -30,15 +30,21 @@ class DepthmapNode:
 
     def __init__(self, depthmap: Depthmap, ref_compl_perc: float = 10.0, max_dist_from_ref: float = 0.5,
                  publish_conv_every_n: int = 10, publisher: Optional[Callable] = None,
-                 volume: Optional[TsdfVolume] = None, prior_from_volume: float = 0.0):
+                 volume: Optional[TsdfVolume] = None, prior_from_volume: float = 0.0, follow_volume: bool = False):
         if prior_from_volume and volume is None:
             raise ValueError("DepthmapNode: prior_from_volume needs a volume")
+        if follow_volume and volume is None:
+            raise ValueError("DepthmapNode: follow_volume needs a volume")
         if not 0.0 <= prior_from_volume <= 1.0:
             raise ValueError("DepthmapNode: prior_from_volume must be in [0, 1] (0 = off)")
         self.depthmap_ = depthmap
         self.volume_ = volume   # when given, every finished keyframe is fused into it (DESIGN.md 4.8)
         # sigma^2 fraction of the new keyframe's prior raycast from volume_ (0 = off)
         self.prior_from_volume_ = float(prior_from_volume)
+        # when set, volume_ is shifted to stay around each keyframe's view before it is fused (DESIGN.md 4.8), and
+        # the surface that leaves it is published as ("volume_spill", (points, intensity or None, normals))
+        self.follow_volume_ = bool(follow_volume)
+        self.ref_depth_range_ = (0.0, 0.0)   # [min_depth, max_depth] of the current keyframe
         self.state_ = TAKE_REFERENCE_FRAME                      # src/depthmap_node.cpp:35
         self.ref_compl_perc_ = float(ref_compl_perc)            # :81, default 10.0
         self.max_dist_from_ref_ = float(max_dist_from_ref)      # :82, default 0.5
@@ -54,6 +60,7 @@ class DepthmapNode:
         if self.state_ == TAKE_REFERENCE_FRAME:
             if self.depthmap_.setReferenceImage(img_8uc1, T_curr_world, min_depth, max_depth):
                 self.state_ = UPDATE                                              # :126-135
+                self.ref_depth_range_ = (float(min_depth), float(max_depth))
                 if self.prior_from_volume_:   # the volume holds every keyframe published so far
                     self.depthmap_.priorFromVolume(self.volume_, self.prior_from_volume_)
         elif self.state_ == UPDATE:
@@ -68,6 +75,8 @@ class DepthmapNode:
             self.num_msgs_ = 0
 
     def denoiseAndPublishResults(self) -> None:
+        if self.follow_volume_:
+            self.followVolume()
         if self.volume_ is not None:
             # the same host map as downloadDenoisedDepthmap, and the keyframe fused from the device copy
             self.depthmap_.fuseDenoisedInto(self.volume_, 0.5, 200)
@@ -76,6 +85,23 @@ class DepthmapNode:
         self.depthmap_.downloadConvergenceMap()                                   # :168
         if self.publisher_:
             self.publisher_("depthmap_and_pointcloud", self.depthmap_)
+
+    def followVolume(self) -> None:
+        """Recentre volume_ on the finished keyframe's view centre -- the camera centre plus the middle of
+        [min_depth, max_depth] along the optical axis -- on every axis where that centre lies more than n / 8 voxels
+        from the grid's centre index, by the whole-voxel difference; the spill is published before the shift."""
+        v = self.volume_
+        T = np.asarray(self.depthmap_.getT_world_ref().data, np.float64).reshape(3, 4)
+        centre = T[:, 3] + 0.5 * (self.ref_depth_range_[0] + self.ref_depth_range_[1]) * T[:, 2]
+        n = np.array(v.dims, np.float64)
+        off = (centre - v.origin.astype(np.float64)) / v.voxel_size - 0.5 * (n - 1.0)
+        d = np.where(np.abs(off) > n / 8.0, np.clip(np.round(off), -(2.0**31 - 1), 2.0**31 - 1), 0.0).astype(np.int64)
+        if not d.any():
+            return
+        if self.publisher_:
+            spill = (v.spillPoints(d), v.spillIntensity(d) if v.intensity else None, v.spillNormals(d))
+            self.publisher_("volume_spill", spill)
+        v.shift(d)
 
     def publishConvergenceMap(self) -> None:
         self.depthmap_.downloadConvergenceMap()                                   # :177
