@@ -348,7 +348,14 @@ int rmd_denoiser_launch_count(rmd_denoiser_t *d, uint64_t *total);
 /* ------------------------------------------------------------ reductions */
 
 /* ImageReducer<T>::sum / countEqual, reduction.cu:81-184.  Device pointer,
- * stride in ELEMENTS (as the reference), legacy default stream, blocking. */
+ * stride in ELEMENTS (as the reference), legacy default stream, blocking.
+ * Only the width x height elements are read, never a row's padding.  Width
+ * or height 0 returns an error.
+ * sum_f32 accumulates in double and rounds once to float: |out - exact| <=
+ * 1/2 ulp(exact) + n 2^-53 sum|x| for n elements (faithful, not always
+ * correctly rounded; with cancellation the second term dominates); an inf
+ * entry gives that inf, +inf with -inf or a NaN entry gives NaN.
+ * sum_i32 wraps exactly like int32 addition. */
 int rmd_reduce_sum_f32(const float *dev_img, size_t stride, size_t width,
                        size_t height, float *out);
 int rmd_reduce_sum_i32(const int32_t *dev_img, size_t stride, size_t width,
@@ -356,7 +363,10 @@ int rmd_reduce_sum_i32(const int32_t *dev_img, size_t stride, size_t width,
 int rmd_reduce_count_eq_i32(const int32_t *dev_img, size_t stride,
                             size_t width, size_t height, int32_t value,
                             size_t *out);
-/* extras the north star asks for (not in the reference) */
+/* extras the north star asks for (not in the reference).
+ * min_max_f32: NaN entries are ignored; an image with no non-NaN entry
+ * returns (+inf, -inf).  Infinities are values like any other, and -0 and +0
+ * compare equal (either may be returned). */
 int rmd_reduce_min_max_f32(const float *dev_img, size_t stride, size_t width,
                            size_t height, float *out_min, float *out_max);
 
