@@ -176,6 +176,44 @@ public:
   std::vector<float> spillIntensity(const int d[3]) { return spill(rmd_volume_spill_intensity, d, 1); }
   std::vector<float> spillNormals(const int d[3]) { return spill(rmd_volume_spill_normals, d, 4); }
 
+  // The mesh a shift by d would drop (call before shift(d)): the triangles of the meshed cubes with a corner leaving
+  // the grid, in mesh() order, indexing xyzw = the subsequence of surfacePoints() they need plus the points that
+  // spill (4 floats per vertex); ids = (i + D0, j + D1, k + D2, axis) per vertex (4 int64), the vertex's identity
+  // across shifts.  Throws for 2^31 or more vertices.
+  void spillMesh(const int d[3], std::vector<float> &xyzw, std::vector<int32_t> &tri, std::vector<int64_t> &ids)
+  {
+    size_t nv = 0, nt = 0;
+    detail::throw_on_error(rmd_volume_spill_mesh(handle_, d, NULL, 0, NULL, 0, NULL, &nv, &nt),
+                           "TsdfVolume: unable to count the spill mesh");
+    xyzw.resize(4 * nv);
+    tri.resize(3 * nt);
+    ids.resize(4 * nv);
+    if(nv || nt)
+      detail::throw_on_error(rmd_volume_spill_mesh(handle_, d, xyzw.data(), nv, tri.data(), nt, ids.data(), &nv, &nt),
+                             "TsdfVolume: unable to extract the spill mesh");
+    xyzw.resize(4 * nv < xyzw.size() ? 4 * nv : xyzw.size());
+    ids.resize(4 * nv < ids.size() ? 4 * nv : ids.size());
+    tri.resize(3 * nt < tri.size() ? 3 * nt : tri.size());
+  }
+  // surfaceIntensity() / surfaceNormals() of the spill mesh's vertices, in their order.
+  std::vector<float> spillMeshIntensity(const int d[3]) { return spill(rmd_volume_spill_mesh_intensity, d, 1); }
+  std::vector<float> spillMeshNormals(const int d[3]) { return spill(rmd_volume_spill_mesh_normals, d, 4); }
+
+  // The ids of surfacePoints() (= mesh() vertices), 4 int64 per point, as spillMesh's.
+  std::vector<int64_t> surfaceIds()
+  {
+    size_t n = 0;
+    detail::throw_on_error(rmd_volume_surface_ids(handle_, NULL, 0, &n), "TsdfVolume: unable to count points");
+    std::vector<int64_t> out(4 * n);
+    if(n)
+      detail::throw_on_error(rmd_volume_surface_ids(handle_, out.data(), n, &n), "TsdfVolume: unable to extract ids");
+    out.resize(4 * n < out.size() ? 4 * n : out.size());
+    return out;
+  }
+
+  // The total offset in voxels, the sum of all shifts.
+  void offset(int64_t D[3]) { detail::throw_on_error(rmd_volume_offset(handle_, D), "TsdfVolume: unable to read the offset"); }
+
   void downloadIntensity(float *host_intensity, float *host_weight)
   {
     detail::throw_on_error(rmd_volume_download_intensity(handle_, host_intensity, host_weight),

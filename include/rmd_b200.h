@@ -661,6 +661,41 @@ int rmd_volume_spill_intensity(rmd_volume_t *v, const int d[3], float *host_inte
                                size_t *count);
 int rmd_volume_spill_normals(rmd_volume_t *v, const int d[3], float *host_nxyz0, size_t capacity, size_t *count);
 
+/* The spill mesh of a shift by d, called BEFORE rmd_volume_shift(v, d)
+ * (DESIGN.md 4.8): the part of rmd_volume_mesh that a shift by d drops, so
+ * that the surface leaving a moving volume can be meshed and joined to the
+ * mesh of what stays.
+ *   A cube (lower corner c < n - 1 per axis) spills when it is meshed (the
+ * mesh's rule) and at least one of its 8 corners lies outside K.  Every meshed
+ * cube either spills or has all corners in K, and is then a cube of the
+ * shifted grid with the same records, case and triangles.
+ *   The vertices V_s are the surface points that spill (rmd_volume_spill_points'
+ * rule) or lie on an edge of a spilling cube (the "seam" points, which also
+ * stay in the grid), as the subsequence of rmd_volume_surface_points in its
+ * order, bit for bit.  The triangles are those of the spilling cubes in
+ * rmd_volume_mesh's order, as int32 indices into V_s.
+ *   host_ids (may be NULL): per vertex 4 int64 (i + D0, j + D1, k + D2, axis),
+ * where (i, j, k) is the point's voxel and D the volume's total offset
+ * (rmd_volume_offset): an identity of the grid edge that survives shifts, by
+ * which the chunks are welded (positions may differ by rounding after a
+ * shift).  It has vertex_capacity entries.
+ *   The mesh's count / capacity / staging contract: NULL buffers with capacity
+ * 0 only count; RMD_ERR_UNSUPPORTED for 2^31 or more vertices.  The intensity
+ * and normals variants return one value per vertex of V_s in its order, with
+ * the spill's contract; the intensity variant returns RMD_ERR_NOT_INITIALISED
+ * without the channel.  Synchronous.  Scratch: the mesh's buffers. */
+int rmd_volume_spill_mesh(rmd_volume_t *v, const int d[3], float *host_xyzw, size_t vertex_capacity, int32_t *host_tri,
+                          size_t tri_capacity, int64_t *host_ids, size_t *n_vertices, size_t *n_triangles);
+int rmd_volume_spill_mesh_intensity(rmd_volume_t *v, const int d[3], float *host_intensity, size_t capacity,
+                                    size_t *count);
+int rmd_volume_spill_mesh_normals(rmd_volume_t *v, const int d[3], float *host_nxyz0, size_t capacity, size_t *count);
+/* The ids (as rmd_volume_spill_mesh's) of rmd_volume_surface_points, and so of
+ * rmd_volume_mesh's vertices, in their order: at most capacity, *count = the
+ * number of points.  Synchronous. */
+int rmd_volume_surface_ids(rmd_volume_t *v, int64_t *host_ids, size_t capacity, size_t *count);
+/* The volume's total offset D in voxels: the sum of its shifts. */
+int rmd_volume_offset(rmd_volume_t *v, int64_t D[3]);
+
 /* ---------------------------------------------------------- device image */
 
 /* DeviceImage<T>(width,height) = cudaMallocPitch, device_image.cuh:37-50 */

@@ -11,7 +11,7 @@ from .api import (ConvergenceStates, DepthmapDenoiser, Depthmap, DeviceImage, Im
                   OPT_RECORD_MATCHES, OPT_KERNEL_VARIANT, OPT_TEX_FRAC_BITS, OPT_DEBUG_TIMELINE, OPT_PINNED_INPUT, OPT_CHAIN_FRAMES, OPT_SEED_MODE_PCT,
                   OPT_TUNE_SPLIT_MAX, OPT_TUNE_SPLIT_MIN_ITEMS, OPT_TUNE_SPLIT_ITEMS_PER_CTA,
                   OPT_TUNE_SPARSE_MAX_SEEDS, OPT_TUNE_HEAVY_MIN_ITEMS, OPT_TUNE_SPLIT_AVG_PCT, OPT_TUNE_PDL, OPT_TUNE_WARP_TILE_SEEDS, OPT_TUNE_GRID_CTAS, OPT_TUNE_CTAS_PER_SM, OPT_TUNE_WARP_TILE_CANDS, OPT_TUNE_RUN_CHUNKS,
-                  VARIANT_STAGED, VARIANT_DIRECT, PRIOR_SIGMA_SQ_FRAC, TsdfVolume, write_ply)
+                  VARIANT_STAGED, VARIANT_DIRECT, PRIOR_SIGMA_SQ_FRAC, SceneMesh, TsdfVolume, write_ply)
 from ._native import device_count
 
 __all__ = [n for n in dir() if not n.startswith("_")]

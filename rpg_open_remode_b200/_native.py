@@ -101,6 +101,11 @@ _SIGNATURES = {
     "rmd_volume_spill_points": (ci, [vp, vp, vp, cs, P(cs)]),
     "rmd_volume_spill_intensity": (ci, [vp, vp, vp, cs, P(cs)]),
     "rmd_volume_spill_normals": (ci, [vp, vp, vp, cs, P(cs)]),
+    "rmd_volume_spill_mesh": (ci, [vp, vp, vp, cs, vp, cs, vp, P(cs), P(cs)]),
+    "rmd_volume_spill_mesh_intensity": (ci, [vp, vp, vp, cs, P(cs)]),
+    "rmd_volume_spill_mesh_normals": (ci, [vp, vp, vp, cs, P(cs)]),
+    "rmd_volume_surface_ids": (ci, [vp, vp, cs, P(cs)]),
+    "rmd_volume_offset": (ci, [vp, vp]),
     "rmd_reduce_sum_f32":(ci, [vp, cs, cs, cs, P(cf)]),
     "rmd_reduce_sum_i32": (ci, [vp, cs, cs, cs, P(ctypes.c_int32)]),
     "rmd_reduce_count_eq_i32": (ci, [vp, cs, cs, cs, ctypes.c_int32, P(cs)]),

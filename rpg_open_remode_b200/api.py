@@ -703,6 +703,59 @@ class TsdfVolume:
         n = self._spill(self._L.rmd_volume_spill_normals, d, capacity, (4,), "TsdfVolume::spillNormals")
         return np.ascontiguousarray(n[:, :3])
 
+    def spillMesh(self, d, vertex_capacity: "int | None" = None, triangle_capacity: "int | None" = None):
+        """The mesh a shift by d would drop (call it before shift(d)): (float32 [n, 4] vertices, int32 [m, 3]
+        triangles, int64 [n, 4] ids).  The triangles are mesh()'s of the meshed cubes with a corner leaving the grid,
+        in mesh() order; the vertices are the subsequence of surfacePoints() made of the points that spill and the
+        seam points those triangles share with the grid that stays.  An id (i + Dx, j + Dy, k + Dz, axis) names the
+        vertex's grid edge across shifts (D = offset); SceneMesh welds by it.  With capacities, at most that many of
+        each.  Raises RmdError (RMD_ERR_UNSUPPORTED) for 2^31 or more vertices."""
+        a = self._offset(d)
+        nv, nt = ctypes.c_size_t(), ctypes.c_size_t()
+        what = "TsdfVolume::spillMesh"
+        if vertex_capacity is None or triangle_capacity is None:
+            check(self._L.rmd_volume_spill_mesh(self._h, a.ctypes.data, None, 0, None, 0, None, ctypes.byref(nv),
+                                                ctypes.byref(nt)), what)
+            vertex_capacity = nv.value if vertex_capacity is None else vertex_capacity
+            triangle_capacity = nt.value if triangle_capacity is None else triangle_capacity
+        verts = np.empty((int(vertex_capacity), 4), np.float32)
+        tris = np.empty((int(triangle_capacity), 3), np.int32)
+        ids = np.empty((int(vertex_capacity), 4), np.int64)
+        check(self._L.rmd_volume_spill_mesh(self._h, a.ctypes.data, verts.ctypes.data if vertex_capacity else None,
+                                            int(vertex_capacity), tris.ctypes.data if triangle_capacity else None,
+                                            int(triangle_capacity), ids.ctypes.data if vertex_capacity else None,
+                                            ctypes.byref(nv), ctypes.byref(nt)), what)
+        m = min(int(vertex_capacity), nv.value)
+        return verts[:m], tris[:min(int(triangle_capacity), nt.value)], ids[:m]
+
+    def spillMeshIntensity(self, d, capacity: "int | None" = None) -> np.ndarray:
+        """surfaceIntensity() of the vertices spillMesh(d) returns, in its order."""
+        return self._spill(self._L.rmd_volume_spill_mesh_intensity, d, capacity, (), "TsdfVolume::spillMeshIntensity")
+
+    def spillMeshNormals(self, d, capacity: "int | None" = None) -> np.ndarray:
+        """float32 [n, 3]: surfaceNormals() of the vertices spillMesh(d) returns, in its order."""
+        n = self._spill(self._L.rmd_volume_spill_mesh_normals, d, capacity, (4,), "TsdfVolume::spillMeshNormals")
+        return np.ascontiguousarray(n[:, :3])
+
+    def surfaceIds(self, capacity: "int | None" = None) -> np.ndarray:
+        """int64 [n, 4]: the id (as spillMesh's) of every surface point (and mesh vertex), in surfacePoints()
+        order."""
+        n = ctypes.c_size_t()
+        if capacity is None:
+            check(self._L.rmd_volume_surface_ids(self._h, None, 0, ctypes.byref(n)), "TsdfVolume::surfaceIds")
+            capacity = n.value
+        out = np.empty((int(capacity), 4), np.int64)
+        check(self._L.rmd_volume_surface_ids(self._h, out.ctypes.data if capacity else None, int(capacity),
+                                             ctypes.byref(n)), "TsdfVolume::surfaceIds")
+        return out[:min(int(capacity), n.value)]
+
+    @property
+    def offset(self) -> np.ndarray:
+        """int64 [3]: the total offset in voxels, the sum of every shift."""
+        D = np.empty(3, np.int64)
+        check(self._L.rmd_volume_offset(self._h, D.ctypes.data), "TsdfVolume::offset")
+        return D
+
     def _download_records(self, fn, what: str):
         """The two halves of a record array (fn: rmd_volume_download[_intensity]), float32 of shape (nz, ny, nx)."""
         nx, ny, nz = self.dims
@@ -781,6 +834,87 @@ def write_ply(path: str, vertices, triangles, intensity=None, normals=None) -> N
         f.write(header.encode("ascii"))
         f.write(v.tobytes())
         f.write(faces.tobytes())
+
+
+class SceneMesh:
+    """One mesh of everything a moving TsdfVolume has seen (DESIGN.md 4.8): the spill mesh of every shift, then the
+    current window's mesh(), welded by vertex id.  Call addSpill(volume, d) before each volume.shift(d); mesh(volume)
+    returns the scene so far and can be called at any time.
+
+    A vertex whose id is pending -- a seam vertex of an earlier chunk whose two voxels are still in the grid -- reuses
+    that vertex; any other vertex is new.  After a chunk, the pending ids with a voxel outside the kept box are dropped
+    (that surface has left the grid, and a voxel that re-enters later starts new vertices), and the chunk's seam
+    vertices become pending.  With intensity / normals, the vertices' spill-mesh and surface intensities / normals
+    are kept as well; a welded vertex keeps those of the chunk that first had it."""
+
+    def __init__(self, intensity: bool = False, normals: bool = False):
+        self.intensity, self.normals = bool(intensity), bool(normals)
+        self._verts, self._tris, self._inten, self._nrm = [], [], [], []
+        self._n = 0                                   # vertices so far
+        self._pend_ids = np.empty((0, 4), np.int64)   # pending ids and their vertex indices
+        self._pend_idx = np.empty(0, np.int64)
+
+    def _weld(self, ids):
+        """(index of each id: the pending vertex's, else a new one from the vertex count on in order; mask of the new
+        ones)."""
+        ids = np.asarray(ids, np.int64).reshape(-1, 4)
+        idx = np.full(len(ids), -1, np.int64)
+        if len(self._pend_ids) and len(ids):
+            _, inv = np.unique(np.concatenate([self._pend_ids, ids]), axis=0, return_inverse=True)
+            inv = inv.reshape(-1)
+            pend_of = np.full(int(inv.max()) + 1, -1, np.int64)
+            pend_of[inv[:len(self._pend_ids)]] = self._pend_idx
+            idx = pend_of[inv[len(self._pend_ids):]]
+        new = idx < 0
+        idx[new] = self._n + np.arange(int(new.sum()), dtype=np.int64)
+        return idx, new
+
+    def _chunk(self, verts, tris, ids, inten, nrm):
+        idx, new = self._weld(ids)
+        if self._n + int(new.sum()) >= 2 ** 31:
+            raise ValueError("SceneMesh: 2^31 or more vertices do not fit int32 indices")
+        tri = idx[np.asarray(tris, np.int64).reshape(-1, 3)].astype(np.int32)
+        chunk = (np.asarray(verts, np.float32).reshape(-1, 4)[new], tri,
+                 None if inten is None else np.asarray(inten, np.float32).reshape(-1)[new],
+                 None if nrm is None else np.asarray(nrm, np.float32).reshape(-1, 3)[new])
+        return idx, new, chunk
+
+    def addSpill(self, volume, d) -> None:
+        """Append the spill mesh of volume's shift by d; call it before volume.shift(d)."""
+        d = np.asarray(d, np.int64).reshape(3)
+        verts, tris, ids = volume.spillMesh(d)
+        inten = volume.spillMeshIntensity(d) if self.intensity else None
+        nrm = volume.spillMeshNormals(d) if self.normals else None
+        idx, new, chunk = self._chunk(verts, tris, ids, inten, nrm)
+        for store, part in zip((self._verts, self._tris, self._inten, self._nrm), chunk):
+            store.append(part)
+        self._n += int(new.sum())
+        # the kept box K in unbounded-grid voxels, as rmd_volume_spill_*: d clamped to [-n, n]
+        n = np.asarray(volume.dims, np.int64)
+        c = np.clip(d, -n, n)
+        D = np.asarray(volume.offset, np.int64)
+        lo, hi = D + np.maximum(c, 0), D + np.where(c < 0, n + c, n)
+        ids = np.asarray(ids, np.int64).reshape(-1, 4)
+        reused = np.isin(self._pend_idx, idx[~new])
+        all_ids = np.concatenate([self._pend_ids[~reused], ids])
+        all_idx = np.concatenate([self._pend_idx[~reused], idx])
+        a = all_ids[:, :3]
+        b = a + np.eye(3, dtype=np.int64)[all_ids[:, 3]]
+        keep = np.all((a >= lo) & (a < hi) & (b >= lo) & (b < hi), axis=1)
+        self._pend_ids, self._pend_idx = all_ids[keep], all_idx[keep]
+
+    def mesh(self, volume):
+        """(float32 [n, 4] vertices, int32 [m, 3] triangles, float32 [n] intensity or None, float32 [n, 3] normals or
+        None) of the chunks added so far and volume's current mesh(), welded alike: the chunks in the order they were
+        added, then the window, each with its new vertices in its own order.  Ready for write_ply.  The accumulated
+        state is not changed."""
+        verts, tris = volume.mesh()
+        inten = volume.surfaceIntensity() if self.intensity else None
+        nrm = volume.surfaceNormals() if self.normals else None
+        _, _, chunk = self._chunk(verts, tris, volume.surfaceIds(), inten, nrm)
+        return (np.concatenate(self._verts + [chunk[0]]), np.concatenate(self._tris + [chunk[1]]),
+                np.concatenate(self._inten + [chunk[2]]) if self.intensity else None,
+                np.concatenate(self._nrm + [chunk[3]]) if self.normals else None)
 
 
 class ImageReducer:

@@ -559,6 +559,149 @@ __global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_mesh_write_kernel(co
   }
 }
 
+// ---------------------------------------------------------------------------------------------- spill mesh
+// Case of cube n when it is meshed and spills from K -- one of its corners, lower corner + {0, 1} per axis, lies
+// outside K -- else 0.
+__device__ __forceinline__ unsigned int spill_cube(const VolumeGrid &g, const VolumeSpillBox &K, unsigned int n,
+                                                   unsigned int n_vox)
+{
+  const unsigned int cube = mesh_cube(g, n, n_vox);
+  if(!cube)
+    return 0u;
+  const unsigned int plane = (unsigned int)g.nx * (unsigned int)g.ny;
+  const int k = (int)(n / plane);
+  const unsigned int rem = n - (unsigned int)k * plane;
+  const int j = (int)(rem / (unsigned int)g.nx);
+  const int i = (int)(rem - (unsigned int)j * (unsigned int)g.nx);
+  const bool leaves = i < K.lo[0] || i + 1 >= K.hi[0] || j < K.lo[1] || j + 1 >= K.hi[1] || k < K.lo[2] ||
+                      k + 1 >= K.hi[2];
+  return leaves ? cube : 0u;
+}
+
+// The spill mesh's vertices of cell c (voxel n): the points that spill from K (spill_mask), and the points that stay
+// whose edge belongs to a spilling cube.  The cubes of edge (a, axis) have lower corners a - du e_u - dw e_w (du, dw
+// in {0, 1}; u, w the other two axes).  Their corners on `axis` are a and a + e_axis, inside K for a staying point, so
+// one of them leaves K only across u or w: that needs a within one voxel of a face of K, and only then are the <= 4
+// cubes tested with mesh_cube.
+__device__ __forceinline__ unsigned int spill_mesh_mask(const VolumeGrid &g, const VolumeSpillBox &K,
+                                                        const SurfaceCell &c, unsigned int n, unsigned int n_vox)
+{
+  const unsigned int spill = spill_mask(K, c);
+  const unsigned int stay = c.mask & ~spill;
+  if(!stay)
+    return spill;
+  const unsigned int plane = (unsigned int)g.nx * (unsigned int)g.ny;
+  unsigned int seam = 0u;
+#pragma unroll
+  for(int axis = 0; axis < 3; ++axis)
+  {
+    if(!(stay & (1u << axis)))
+      continue;
+    const int pu = axis == 0 ? c.j : c.i, pw = axis == 2 ? c.j : c.k;
+    const int lu = axis == 0 ? K.lo[1] : K.lo[0], hu = axis == 0 ? K.hi[1] : K.hi[0];
+    const int lw = axis == 2 ? K.lo[1] : K.lo[2], hw = axis == 2 ? K.hi[1] : K.hi[2];
+    const unsigned int su = axis == 0 ? (unsigned int)g.nx : 1u, sw = axis == 2 ? (unsigned int)g.nx : plane;
+    if(pu > lu && pu + 1 < hu && pw > lw && pw + 1 < hw)   // every cube of the edge lies inside K
+      continue;
+    bool hit = false;
+#pragma unroll 1
+    for(int q = 0; q < 4 && !hit; ++q)
+    {
+      const int du = q & 1, dw = q >> 1;
+      const int cu = pu - du, cw = pw - dw;
+      if(cu < 0 || cw < 0 || !(cu < lu || cu + 1 >= hu || cw < lw || cw + 1 >= hw))
+        continue;
+      hit = mesh_cube(g, n - (unsigned int)du * su - (unsigned int)dw * sw, n_vox) != 0u;
+    }
+    seam |= hit ? (1u << axis) : 0u;
+  }
+  return spill | seam;
+}
+
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_spill_mesh_count_kernel(const VolumeSurfaceParams P,
+                                                                                    const VolumeSpillBox K)
+{
+  const unsigned int n_vox = grid_voxels(P.g);
+  count_block(P.b, [&](unsigned int n) {
+    return (unsigned int)__popc(spill_mesh_mask(P.g, K, surface_cell(P.g, n, n_vox), n, n_vox));
+  });
+}
+
+// volume_spill_write_kernel on the spill mesh's vertices.  With P.keys, also every vertex's key 3 * voxel + axis, for
+// all *total vertices whatever the capacity (as the surface kernel's KEYS instance), for mesh_vertex.
+template<bool INTENSITY, bool NORMALS>
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_spill_mesh_write_kernel(const VolumeSurfaceParams P,
+                                                                                    const VolumeSpillBox K)
+{
+  __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
+  const unsigned int n_vox = grid_voxels(P.g);
+  const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
+  unsigned long long rank = P.b.block_offsets[blockIdx.x];
+  for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
+  {
+    const unsigned int n = base + r * VOLUME_SURF_BLOCK;
+    SurfaceCell c = surface_cell(P.g, n, n_vox);
+    c.mask = spill_mesh_mask(P.g, K, c, n, n_vox);
+    unsigned int all;
+    unsigned long long slot = round_slot(rank, __popc(c.mask), warp_off, all);
+#pragma unroll
+    for(int axis = 0; axis < 3; ++axis)
+    {
+      if(!(c.mask & (1u << axis)))
+        continue;
+      if(slot < P.capacity)
+      {
+        if(INTENSITY)
+          P.intensity[slot] = surface_intensity(P, c, n, axis);
+        else if(NORMALS)
+          P.normals[slot] = surface_normal(P.g, c, axis);
+        else
+          P.out[slot] = surface_point(P.g, c, axis);
+      }
+      if(P.keys)
+        P.keys[slot] = 3ull * n + axis;
+      ++slot;
+    }
+    rank += all;
+    __syncthreads();   // warp_off is reused by the next round
+  }
+}
+
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_spill_tri_count_kernel(const VolumeMeshParams P,
+                                                                                   const VolumeSpillBox K)
+{
+  const unsigned int n_vox = grid_voxels(P.g);
+  count_block(P.b, [&](unsigned int n) { return (unsigned int)RMD_MC_NTRI[spill_cube(P.g, K, n, n_vox)]; });
+}
+
+// volume_mesh_write_kernel on the cubes that spill from K; P's point offsets, total and keys are the spill mesh's
+// vertices', so that mesh_vertex finds an index into them.
+__global__ void __launch_bounds__(VOLUME_SURF_BLOCK) volume_spill_tri_write_kernel(const VolumeMeshParams P,
+                                                                                   const VolumeSpillBox K)
+{
+  __shared__ unsigned int warp_off[VOLUME_SURF_BLOCK / 32];
+  const unsigned int n_vox = grid_voxels(P.g);
+  const unsigned int base = blockIdx.x * VOLUME_SURF_VOXELS + threadIdx.x;
+  unsigned long long rank = P.b.block_offsets[blockIdx.x];
+  for(int r = 0; r < VOLUME_SURF_ROUNDS; ++r)
+  {
+    const unsigned int n = base + r * VOLUME_SURF_BLOCK;
+    const unsigned int cube = spill_cube(P.g, K, n, n_vox);
+    const unsigned int cnt = RMD_MC_NTRI[cube];
+    unsigned int all;
+    unsigned long long slot = round_slot(rank, cnt, warp_off, all);
+    for(unsigned int q = 0; q < cnt && slot < P.capacity; ++q, ++slot)
+    {
+      int *t = P.tri + 3 * slot;
+      t[0] = mesh_vertex(P, n, RMD_MC_TRIS[cube][3 * q + 0]);
+      t[1] = mesh_vertex(P, n, RMD_MC_TRIS[cube][3 * q + 1]);
+      t[2] = mesh_vertex(P, n, RMD_MC_TRIS[cube][3 * q + 2]);
+    }
+    rank += all;
+    __syncthreads();   // warp_off is reused by the next round
+  }
+}
+
 // --------------------------------------------------------------------------------------------- raycast
 // Trilinear interpolation of the records rec (g.vox or the intensity records, indexed alike) at grid coordinates
 // (gx, gy, gz), in x, then y, then z; false if a corner lies outside the grid or has weight 0.
@@ -855,6 +998,41 @@ cudaError_t launch_volume_spill_write(const VolumeSurfaceParams &P, const Volume
     volume_spill_write_kernel<false, true><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
   else
     volume_spill_write_kernel<false, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_spill_mesh_count(const VolumeSurfaceParams &P, const VolumeSpillBox &K, cudaStream_t stream)
+{
+  volume_spill_mesh_count_kernel<<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  cudaError_t err = cudaGetLastError();
+  if(err != cudaSuccess) return err;
+  volume_surface_scan_kernel<<<1, VOLUME_SCAN_BLOCK, 0, stream>>>(P.b);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_spill_mesh_write(const VolumeSurfaceParams &P, const VolumeSpillBox &K, cudaStream_t stream)
+{
+  if(P.intensity)
+    volume_spill_mesh_write_kernel<true, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  else if(P.normals)
+    volume_spill_mesh_write_kernel<false, true><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  else
+    volume_spill_mesh_write_kernel<false, false><<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_spill_tri_count(const VolumeMeshParams &P, const VolumeSpillBox &K, cudaStream_t stream)
+{
+  volume_spill_tri_count_kernel<<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  cudaError_t err = cudaGetLastError();
+  if(err != cudaSuccess) return err;
+  volume_surface_scan_kernel<<<1, VOLUME_SCAN_BLOCK, 0, stream>>>(P.b);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_spill_tri_write(const VolumeMeshParams &P, const VolumeSpillBox &K, cudaStream_t stream)
+{
+  volume_spill_tri_write_kernel<<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
   return cudaGetLastError();
 }
 

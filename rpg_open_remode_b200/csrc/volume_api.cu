@@ -78,15 +78,18 @@ enum SurfaceOutput { SURFACE_POINTS, SURFACE_INTENSITY, SURFACE_NORMALS };
 
 // The surface points' count pass and scan, one host read of the count, then for min(count, capacity) points their
 // write pass (same blocks and ranks): positions (float4), intensities (float) or normals (float4).  With a spill box,
-// only the points that spill from it.  host: staged in v->stage and copied to out.  Synchronous.
+// only the points that spill from it, or with spill_mesh the spill mesh's vertices.  host: staged in v->stage and
+// copied to out.  Synchronous.
 int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, bool host, SurfaceOutput kind,
-                   const VolumeSpillBox *spill = NULL)
+                   const VolumeSpillBox *spill = NULL, bool spill_mesh = false)
 {
   const bool intensity = kind == SURFACE_INTENSITY;
   VolumeSurfaceParams P;
   int rc = volume_surface_params(v, P);
   if(rc) return rc;
-  if(spill)
+  if(spill && spill_mesh)
+    RMD_CUDA_TRY(launch_volume_spill_mesh_count(P, *spill, v->stream));
+  else if(spill)
     RMD_CUDA_TRY(launch_volume_spill_count(P, *spill, v->stream));
   else
     RMD_CUDA_TRY(launch_volume_surface_count(P, v->stream));
@@ -115,7 +118,9 @@ int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, boo
     P.normals = static_cast<float4*>(dst);
   else
     P.out = static_cast<float4*>(dst);
-  if(spill)
+  if(spill && spill_mesh)
+    RMD_CUDA_TRY(launch_volume_spill_mesh_write(P, *spill, v->stream));
+  else if(spill)
     RMD_CUDA_TRY(launch_volume_spill_write(P, *spill, v->stream));
   else
     RMD_CUDA_TRY(launch_volume_surface_write(P, v->stream));
@@ -128,10 +133,10 @@ int volume_surface(rmd_volume *v, void *out, size_t capacity, size_t *count, boo
 // The mesh: both count passes and scans, one host read of the two totals, then -- for what the capacities ask --
 // the surface points (with their keys when triangles are wanted) and the triangles.  host: min(count, capacity)
 // of each are staged in the volume's buffers and copied to xyzw / tri.  Synchronous.
-int volume_mesh(rmd_volume *v, void *xyzw, size_t vertex_capacity, int32_t *tri, size_t tri_capacity,
-                size_t *n_vertices, size_t *n_triangles, bool host, const char *what)
+// The surface points' and the triangles' pass parameters on v's grid, with the per-block offsets and totals of both
+// (allocated on first use).
+int volume_mesh_params(rmd_volume *v, VolumeSurfaceParams &S, VolumeMeshParams &M)
 {
-  VolumeSurfaceParams S;
   int rc = volume_surface_params(v, S);
   if(rc) return rc;
   if(!v->tri_offsets)
@@ -139,7 +144,6 @@ int volume_mesh(rmd_volume *v, void *xyzw, size_t vertex_capacity, int32_t *tri,
     RMD_CUDA_TRY(cudaMalloc(&v->tri_offsets, sizeof(unsigned long long) * S.b.n_blocks));
     RMD_CUDA_TRY(cudaMalloc(&v->tri_total, sizeof(unsigned long long)));
   }
-  VolumeMeshParams M;
   memset(&M, 0, sizeof(M));
   M.g = v->g;
   M.point_offsets = v->surf_offsets;
@@ -147,6 +151,16 @@ int volume_mesh(rmd_volume *v, void *xyzw, size_t vertex_capacity, int32_t *tri,
   M.b.block_offsets = v->tri_offsets;
   M.b.total = v->tri_total;
   M.b.n_blocks = S.b.n_blocks;
+  return 0;
+}
+
+int volume_mesh(rmd_volume *v, void *xyzw, size_t vertex_capacity, int32_t *tri, size_t tri_capacity,
+                size_t *n_vertices, size_t *n_triangles, bool host, const char *what)
+{
+  VolumeSurfaceParams S;
+  VolumeMeshParams M;
+  int rc = volume_mesh_params(v, S, M);
+  if(rc) return rc;
   RMD_CUDA_TRY(launch_volume_surface_count(S, v->stream));
   RMD_CUDA_TRY(launch_volume_mesh_count(M, v->stream));
   unsigned long long nv = 0, nt = 0;
@@ -361,6 +375,79 @@ int volume_spill(const char *what, rmd_volume_t *v, const int d[3], void *host_o
   return volume_surface(v, host_out, capacity, count, true, kind, &K);
 }
 
+// The first m entries of ids hold the keys 3 * voxel + axis of m vertices (as uint64); they become the vertices'
+// ids (i + D0, j + D1, k + D2, axis), 4 per vertex, in place -- from the back, so that no key is overwritten before
+// it is read.
+void keys_to_ids(const rmd_volume *v, int64_t *ids, size_t m)
+{
+  const uint64_t nx = (uint64_t)v->g.nx, ny = (uint64_t)v->g.ny;
+  for(size_t q = m; q-- > 0;)
+  {
+    const uint64_t key = (uint64_t)ids[q], vox = key / 3, row = vox / nx;
+    ids[4 * q + 0] = (int64_t)(vox - row * nx) + v->D[0];
+    ids[4 * q + 1] = (int64_t)(row % ny) + v->D[1];
+    ids[4 * q + 2] = (int64_t)(row / ny) + v->D[2];
+    ids[4 * q + 3] = (int64_t)(key - 3 * vox);
+  }
+}
+
+// rmd_volume_spill_mesh: both count passes and scans on K, one host read of the two totals, then -- for what the
+// capacities ask -- the vertices (with their keys when triangles or ids are wanted) and the triangles, staged in the
+// volume's buffers and copied to the host; ids from the keys.  Synchronous.
+int volume_spill_mesh(rmd_volume *v, const VolumeSpillBox &K, float *xyzw, size_t vertex_capacity, int32_t *tri,
+                      size_t tri_capacity, int64_t *ids, size_t *n_vertices, size_t *n_triangles, const char *what)
+{
+  VolumeSurfaceParams S;
+  VolumeMeshParams M;
+  int rc = volume_mesh_params(v, S, M);
+  if(rc) return rc;
+  RMD_CUDA_TRY(launch_volume_spill_mesh_count(S, K, v->stream));
+  RMD_CUDA_TRY(launch_volume_spill_tri_count(M, K, v->stream));
+  unsigned long long nv = 0, nt = 0;
+  RMD_CUDA_TRY(cudaMemcpyAsync(&nv, v->surf_total, sizeof(nv), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaMemcpyAsync(&nt, v->tri_total, sizeof(nt), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  *n_vertices = (size_t)nv;
+  *n_triangles = (size_t)nt;
+  if(nv >= (1ull << 31))
+    return fail(RMD_ERR_UNSUPPORTED, (std::string(what) + ": 2^31 or more vertices do not fit int32 indices").c_str());
+  const size_t mv = nv < vertex_capacity ? (size_t)nv : vertex_capacity;
+  const size_t mt = nt < tri_capacity ? (size_t)nt : tri_capacity;
+  if(!mv && !mt)
+    return 0;
+  rc = volume_grow(&v->stage, &v->stage_cap, mv * sizeof(float4));
+  if(!rc) rc = volume_grow(&v->tri_stage, &v->tri_stage_cap, 3 * mt);
+  if(rc) return rc;
+  S.out = reinterpret_cast<float4*>(v->stage);
+  S.capacity = mv;
+  const bool keys = mt || (ids && mv);
+  if(keys)
+  {
+    // every vertex's key, whatever the vertex capacity: triangles may index vertices that are not returned
+    rc = volume_grow(&v->keys, &v->keys_cap, (size_t)nv);
+    if(rc) return rc;
+    S.keys = v->keys;
+  }
+  RMD_CUDA_TRY(launch_volume_spill_mesh_write(S, K, v->stream));
+  if(mt)
+  {
+    M.keys = v->keys;
+    M.tri = v->tri_stage;
+    M.capacity = mt;
+    RMD_CUDA_TRY(launch_volume_spill_tri_write(M, K, v->stream));
+  }
+  if(mv)
+    RMD_CUDA_TRY(cudaMemcpyAsync(xyzw, v->stage, mv * sizeof(float4), cudaMemcpyDeviceToHost, v->stream));
+  if(mt)
+    RMD_CUDA_TRY(cudaMemcpyAsync(tri, v->tri_stage, mt * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, v->stream));
+  if(ids && mv)
+    RMD_CUDA_TRY(cudaMemcpyAsync(ids, v->keys, mv * sizeof(uint64_t), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  if(ids)
+    keys_to_ids(v, ids, mv);
+  return 0;
+}
+
 // origin + (float)D * s, one rounding per operation as the kernels' voxel_coord (volatile: no contraction)
 float shifted_origin(float origin, long long D, float s)
 {
@@ -535,6 +622,72 @@ int rmd_volume_spill_intensity(rmd_volume_t *v, const int d[3], float *host_inte
 int rmd_volume_spill_normals(rmd_volume_t *v, const int d[3], float *host_nxyz0, size_t capacity, size_t *count)
 {
   return volume_spill("rmd_volume_spill_normals", v, d, host_nxyz0, capacity, count, SURFACE_NORMALS);
+}
+
+int rmd_volume_spill_mesh(rmd_volume_t *v, const int d[3], float *host_xyzw, size_t vertex_capacity, int32_t *host_tri,
+                          size_t tri_capacity, int64_t *host_ids, size_t *n_vertices, size_t *n_triangles)
+{
+  const char *what = "rmd_volume_spill_mesh";
+  VOLUME_REQUIRE(v && d && n_vertices && n_triangles && (host_xyzw || vertex_capacity == 0) &&
+                 (host_tri || tri_capacity == 0), "null argument");
+  DeviceGuard guard(v->device);
+  return volume_spill_mesh(v, spill_box(v, d), host_xyzw, vertex_capacity, host_tri, tri_capacity, host_ids,
+                           n_vertices, n_triangles, what);
+}
+
+int rmd_volume_spill_mesh_intensity(rmd_volume_t *v, const int d[3], float *host_intensity, size_t capacity,
+                                    size_t *count)
+{
+  const char *what = "rmd_volume_spill_mesh_intensity";
+  VOLUME_REQUIRE(v && d && count && (host_intensity || capacity == 0), "null argument");
+  if(!v->col)
+    return no_intensity(what);
+  DeviceGuard guard(v->device);
+  const VolumeSpillBox K = spill_box(v, d);
+  return volume_surface(v, host_intensity, capacity, count, true, SURFACE_INTENSITY, &K, true);
+}
+
+int rmd_volume_spill_mesh_normals(rmd_volume_t *v, const int d[3], float *host_nxyz0, size_t capacity, size_t *count)
+{
+  const char *what = "rmd_volume_spill_mesh_normals";
+  VOLUME_REQUIRE(v && d && count && (host_nxyz0 || capacity == 0), "null argument");
+  DeviceGuard guard(v->device);
+  const VolumeSpillBox K = spill_box(v, d);
+  return volume_surface(v, host_nxyz0, capacity, count, true, SURFACE_NORMALS, &K, true);
+}
+
+int rmd_volume_surface_ids(rmd_volume_t *v, int64_t *host_ids, size_t capacity, size_t *count)
+{
+  RMD_REQUIRE(v && count && (host_ids || capacity == 0), "rmd_volume_surface_ids: null argument");
+  DeviceGuard guard(v->device);
+  VolumeSurfaceParams P;
+  int rc = volume_surface_params(v, P);
+  if(rc) return rc;
+  RMD_CUDA_TRY(launch_volume_surface_count(P, v->stream));
+  unsigned long long total = 0;
+  RMD_CUDA_TRY(cudaMemcpyAsync(&total, v->surf_total, sizeof(total), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  *count = (size_t)total;
+  const size_t m = *count < capacity ? *count : capacity;
+  if(!m)
+    return 0;
+  // the mesh path's key pass with no point output: every point's key
+  rc = volume_grow(&v->keys, &v->keys_cap, (size_t)total);
+  if(rc) return rc;
+  P.keys = v->keys;
+  RMD_CUDA_TRY(launch_volume_surface_write(P, v->stream));
+  RMD_CUDA_TRY(cudaMemcpyAsync(host_ids, v->keys, m * sizeof(uint64_t), cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  keys_to_ids(v, host_ids, m);
+  return 0;
+}
+
+int rmd_volume_offset(rmd_volume_t *v, int64_t D[3])
+{
+  RMD_REQUIRE(v && D, "rmd_volume_offset: null argument");
+  for(int a = 0; a < 3; ++a)
+    D[a] = v->D[a];
+  return 0;
 }
 
 int rmd_volume_enable_intensity(rmd_volume_t *v)

@@ -17,7 +17,7 @@ from typing import Callable, List, Optional
 
 import numpy as np
 
-from .api import PRIOR_SIGMA_SQ_FRAC, SE3, Depthmap, SeedMatrix, TsdfVolume
+from .api import PRIOR_SIGMA_SQ_FRAC, SE3, Depthmap, SceneMesh, SeedMatrix, TsdfVolume
 
 UPDATE, TAKE_REFERENCE_FRAME = 0, 1   # rmd::ProcessingStates::State, include/rmd/depthmap_node.h:32-36
 
@@ -30,11 +30,14 @@ class DepthmapNode:
 
     def __init__(self, depthmap: Depthmap, ref_compl_perc: float = 10.0, max_dist_from_ref: float = 0.5,
                  publish_conv_every_n: int = 10, publisher: Optional[Callable] = None,
-                 volume: Optional[TsdfVolume] = None, prior_from_volume: float = 0.0, follow_volume: bool = False):
+                 volume: Optional[TsdfVolume] = None, prior_from_volume: float = 0.0, follow_volume: bool = False,
+                 scene_mesh: Optional[SceneMesh] = None):
         if prior_from_volume and volume is None:
             raise ValueError("DepthmapNode: prior_from_volume needs a volume")
         if follow_volume and volume is None:
             raise ValueError("DepthmapNode: follow_volume needs a volume")
+        if scene_mesh is not None and not follow_volume:
+            raise ValueError("DepthmapNode: scene_mesh needs follow_volume=True")
         if not 0.0 <= prior_from_volume <= 1.0:
             raise ValueError("DepthmapNode: prior_from_volume must be in [0, 1] (0 = off)")
         self.depthmap_ = depthmap
@@ -44,6 +47,9 @@ class DepthmapNode:
         # when set, volume_ is shifted to stay around each keyframe's view before it is fused (DESIGN.md 4.8), and
         # the surface that leaves it is published as ("volume_spill", (points, intensity or None, normals))
         self.follow_volume_ = bool(follow_volume)
+        # when given, the spill mesh of every shift is added to it, so that scene_mesh.mesh(volume) meshes the whole
+        # traversed scene
+        self.scene_mesh_ = scene_mesh
         self.ref_depth_range_ = (0.0, 0.0)   # [min_depth, max_depth] of the current keyframe
         self.state_ = TAKE_REFERENCE_FRAME                      # src/depthmap_node.cpp:35
         self.ref_compl_perc_ = float(ref_compl_perc)            # :81, default 10.0
@@ -101,6 +107,8 @@ class DepthmapNode:
         if self.publisher_:
             spill = (v.spillPoints(d), v.spillIntensity(d) if v.intensity else None, v.spillNormals(d))
             self.publisher_("volume_spill", spill)
+        if self.scene_mesh_ is not None:
+            self.scene_mesh_.addSpill(v, d)
         v.shift(d)
 
     def publishConvergenceMap(self) -> None:

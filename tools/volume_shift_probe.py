@@ -1,16 +1,19 @@
-"""Timing of the moving TSDF volume (DESIGN.md 4.8, 6): rmd_volume_shift and the three spills at 256^3 and 512^3,
-with the intensity channel, on a volume fused from one ground-truth VGA frame.
+"""Timing of the moving TSDF volume (DESIGN.md 4.8, 6): rmd_volume_shift, the three spills and the spill mesh (with
+its intensities and normals) at 256^3 and 512^3, with the intensity channel, on a volume fused from one ground-truth
+VGA frame.
 
 CUDA events on the volume's stream, warm (one untimed call each first), the variants alternating within each of
 `--reps` rounds; the median per variant.  The shift moves (8 + 8) B per voxel per channel; it is reported as bytes
 over time against the H100 SXM's 3.35 TB/s data-sheet figure.  A spill reads what the surface passes read and is
-reported against rmd_volume_surface_points / _intensity / _normals of the same grid.
+reported against rmd_volume_surface_points / _intensity / _normals of the same grid; the spill mesh against
+rmd_volume_mesh, its intensities and normals against the surface calls of the same kind.
 
     python tools/volume_shift_probe.py [--reps 20]
 """
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 import numpy as np
@@ -40,6 +43,11 @@ def main():
     cam = rmd.PinholeCamera(*seq.camera)
     stream = torch.cuda.Stream()
     out = {"gpu": torch.cuda.get_device_name(0), "reps": args.reps}
+    try:
+        out["power_limit"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"],
+                                            capture_output=True, text=True, timeout=60).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        out["power_limit"] = "unknown"
     for n in (256, 512):
         lo, hi = pts.min(0), pts.max(0)
         s = float(((hi - lo) / (n - 1 - 16)).max())
@@ -57,6 +65,10 @@ def main():
             "surface_points": lambda: v.surfacePoints(),
             "surface_intensity": lambda: v.surfaceIntensity(),
             "surface_normals": lambda: v.surfaceNormals(),
+            "mesh": lambda: v.mesh(),
+            "spill_mesh": lambda: v.spillMesh(ds),
+            "spill_mesh_intensity": lambda: v.spillMeshIntensity(ds),
+            "spill_mesh_normals": lambda: v.spillMeshNormals(ds),
         }
         for fn in ops.values():
             fn()
@@ -78,6 +90,13 @@ def main():
         row["shift_of_peak"] = round(row["shift_TBps"] / HBM_TBPS, 3)
         for kind in ("points", "intensity", "normals"):
             row[f"spill_over_surface_{kind}"] = round(med[f"spill_{kind}"] / med[f"surface_{kind}"], 3)
+        row["spill_mesh_over_mesh"] = round(med["spill_mesh"] / med["mesh"], 3)
+        for kind in ("intensity", "normals"):
+            row[f"spill_mesh_over_surface_{kind}"] = round(med[f"spill_mesh_{kind}"] / med[f"surface_{kind}"], 3)
+        sv, st, _ = v.spillMesh(ds)
+        mv, mt = v.mesh()
+        row["spill_mesh_vertices_triangles"] = [len(sv), len(st)]
+        row["mesh_vertices_triangles"] = [len(mv), len(mt)]
         row["spill_points"] = len(v.spillPoints(ds))
         row["surface_points"] = len(v.surfacePoints())
         out[f"{n}^3"] = row
