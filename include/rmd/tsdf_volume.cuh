@@ -214,6 +214,41 @@ public:
   // The total offset in voxels, the sum of all shifts.
   void offset(int64_t D[3]) { detail::throw_on_error(rmd_volume_offset(handle_, D), "TsdfVolume: unable to read the offset"); }
 
+  // Brick store: shift() then keeps the 8x8x8 bricks that leave the grid with a known voxel and restores the voxels
+  // that re-enter (shift(d) then shift(-d) is lossless); each such shift synchronises the volume's stream once.
+  void enableStore() { detail::throw_on_error(rmd_volume_enable_store(handle_), "TsdfVolume: unable to enable the store"); }
+  // The number of stored bricks and the device bytes of the store's pool.
+  void storeInfo(size_t *bricks, size_t *bytes)
+  {
+    detail::throw_on_error(rmd_volume_store_info(handle_, bricks, bytes), "TsdfVolume: unable to read the store");
+  }
+  // The stored bricks in ascending (z, y, x): 3 int64 coordinates and 512 records (x fastest) per brick; voxels inside
+  // the grid are (0, 0).  intensity / intensity_weight (NULL: not wanted) need the intensity channel.
+  void downloadStore(std::vector<int64_t> &coords, std::vector<float> &tsdf, std::vector<float> &weight,
+                     std::vector<float> *intensity = NULL, std::vector<float> *intensity_weight = NULL)
+  {
+    size_t n = 0;
+    detail::throw_on_error(rmd_volume_download_store(handle_, NULL, NULL, NULL, NULL, NULL, 0, &n),
+                           "TsdfVolume: unable to count the stored bricks");
+    coords.resize(3 * n);
+    tsdf.resize(512 * n);
+    weight.resize(512 * n);
+    if(intensity) intensity->resize(512 * n);
+    if(intensity_weight) intensity_weight->resize(512 * n);
+    if(n)
+      detail::throw_on_error(rmd_volume_download_store(handle_, coords.data(), tsdf.data(), weight.data(),
+                                                       intensity ? intensity->data() : NULL,
+                                                       intensity_weight ? intensity_weight->data() : NULL, n, &n),
+                             "TsdfVolume: unable to download the store");
+  }
+  // Replaces the store with n bricks laid out as downloadStore's (intensity pair optional).
+  void uploadStore(const int64_t *coords, const float *tsdf, const float *weight, size_t n,
+                   const float *intensity = NULL, const float *intensity_weight = NULL)
+  {
+    detail::throw_on_error(rmd_volume_upload_store(handle_, coords, tsdf, weight, intensity, intensity_weight, n),
+                           "TsdfVolume: unable to upload the store");
+  }
+
   void downloadIntensity(float *host_intensity, float *host_weight)
   {
     detail::throw_on_error(rmd_volume_download_intensity(handle_, host_intensity, host_weight),

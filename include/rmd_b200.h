@@ -640,7 +640,10 @@ int rmd_volume_raycast_normals(rmd_volume_t *v, int width, int height, float fx,
  * grid, and work already enqueued keeps reading the records it was launched
  * with (the rays of rmd_volume_prior_seeds included: the volume's stream
  * waits for them, so the next shift cannot overwrite what they read).
- * download, upload and reset act on the current grid.
+ * download, upload and reset act on the current grid.  With the brick store
+ * (rmd_volume_enable_store, below) the shift also keeps what leaves and
+ * restores what re-enters, and synchronises the volume's stream once when it
+ * meets a brick not yet stored.
  * RMD_ERR_INVALID_ARGUMENT: null handle or pointer, a total offset that
  * overflows 64 bits or an origin that would not be finite; the volume is then
  * unchanged. */
@@ -695,6 +698,66 @@ int rmd_volume_spill_mesh_normals(rmd_volume_t *v, const int d[3], float *host_n
 int rmd_volume_surface_ids(rmd_volume_t *v, int64_t *host_ids, size_t capacity, size_t *count);
 /* The volume's total offset D in voxels: the sum of its shifts. */
 int rmd_volume_offset(rmd_volume_t *v, int64_t D[3]);
+
+/* Brick store (DESIGN.md 4.8): an opt-in sparse store in device memory that
+ * keeps the voxels a moving volume leaves and gives them back when they
+ * re-enter, so that the map -- the store plus the window -- loses nothing.
+ *   A brick is 8 x 8 x 8 voxels of the unbounded grid: window voxel (i, j, k)
+ * is voxel u = (i, j, k) + D (rmd_volume_offset), in brick floor(u / 8) per
+ * axis.  A stored brick holds 512 (tsdf, weight) records, x fastest, and with
+ * the intensity channel 512 (intensity, weight) records.
+ *   On rmd_volume_shift(v, d), every brick with a voxel in the pre-shift
+ * window outside the kept box K (rmd_volume_spill_points; empty when
+ * |d| >= n) is visited: a stored brick gets all its leaving voxels written; a
+ * brick not stored is stored when one of its leaving voxels has weight > 0 --
+ * its leaving voxels written, its other voxels (0, 0) -- and skipped
+ * otherwise.  Then every voxel that enters the window (its pre-shift source
+ * lay outside the grid) takes its brick's stored records, or (0, 0) when the
+ * brick is not stored.  So every voxel of the unbounded grid is in the window,
+ * or holds its last value in the store, or is unknown, and shift(d) followed
+ * by shift(-d) gives back the window bit for bit.  A stored brick stays stored
+ * when its voxels are back in the window; its copies of them are stale and
+ * never read.
+ *   Integration, extraction, raycasts, the prior and the spills act on the
+ * window as without the store.  rmd_volume_reset also empties the store (its
+ * memory stays allocated until rmd_volume_destroy); download and upload act on
+ * the window; rmd_volume_enable_intensity gives bricks already stored zeroed
+ * colour records.
+ *
+ * rmd_volume_enable_store turns the store on (nothing is allocated until a
+ * shift stores a brick); a second call does nothing.  From then on
+ * rmd_volume_shift reads one flag per new candidate brick back to the host, so
+ * it synchronises the volume's stream once when such a brick exists; the pool
+ * grows by doubling.  A shift whose pool cannot grow returns
+ * cudaErrorMemoryAllocation, and one whose total offset plus the grid size
+ * overflows 64 bits RMD_ERR_INVALID_ARGUMENT; the volume (window, offset and
+ * store) is then unchanged.  RMD_ERR_INVALID_ARGUMENT: null handle, or an
+ * offset already that large.
+ *
+ * The other entry points return RMD_ERR_NOT_INITIALISED on a volume without
+ * the store, and RMD_ERR_INVALID_ARGUMENT for a null handle or pointer. */
+int rmd_volume_enable_store(rmd_volume_t *v);
+/* The number of stored bricks and the bytes of device memory the store's
+ * pool holds.  Either output may be NULL. */
+int rmd_volume_store_info(rmd_volume_t *v, size_t *bricks, size_t *bytes);
+/* The stored bricks in ascending (z, y, x) brick coordinate: per brick 3
+ * int64 (bx, by, bz) to host_coords and 512 records, x fastest, to the record
+ * arrays; a voxel inside the current window is returned as (0, 0), since the
+ * window holds it.  *count = the number of bricks, of which min(count,
+ * capacity) are written; NULL host_coords with capacity 0 only counts.  Any
+ * record array may be NULL (not written); the intensity ones return
+ * RMD_ERR_NOT_INITIALISED without the channel.  Synchronous. */
+int rmd_volume_download_store(rmd_volume_t *v, int64_t *host_coords, float *host_tsdf, float *host_weight,
+                              float *host_intensity, float *host_intensity_weight, size_t capacity, size_t *count);
+/* Test / checkpoint hook (like rmd_volume_upload): replaces the store with
+ * count bricks laid out as rmd_volume_download_store's.  Voxels inside the
+ * window are ignored.  host_intensity and host_intensity_weight come together
+ * or are both NULL (zeroed colour records); RMD_ERR_NOT_INITIALISED when given
+ * without the channel.  RMD_ERR_INVALID_ARGUMENT: null arrays with count > 0,
+ * a duplicate brick, a coordinate outside [-2^60, 2^60).  Synchronous. */
+int rmd_volume_upload_store(rmd_volume_t *v, const int64_t *host_coords, const float *host_tsdf,
+                            const float *host_weight, const float *host_intensity,
+                            const float *host_intensity_weight, size_t count);
 
 /* ---------------------------------------------------------- device image */
 

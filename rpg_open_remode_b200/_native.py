@@ -106,6 +106,10 @@ _SIGNATURES = {
     "rmd_volume_spill_mesh_normals": (ci, [vp, vp, vp, cs, P(cs)]),
     "rmd_volume_surface_ids": (ci, [vp, vp, cs, P(cs)]),
     "rmd_volume_offset": (ci, [vp, vp]),
+    "rmd_volume_enable_store": (ci, [vp]),
+    "rmd_volume_store_info": (ci, [vp, P(cs), P(cs)]),
+    "rmd_volume_download_store": (ci, [vp, vp, vp, vp, vp, vp, cs, P(cs)]),
+    "rmd_volume_upload_store": (ci, [vp, vp, vp, vp, vp, vp, cs]),
     "rmd_reduce_sum_f32":(ci, [vp, cs, cs, cs, P(cf)]),
     "rmd_reduce_sum_i32": (ci, [vp, cs, cs, cs, P(ctypes.c_int32)]),
     "rmd_reduce_count_eq_i32": (ci, [vp, cs, cs, cs, ctypes.c_int32, P(cs)]),

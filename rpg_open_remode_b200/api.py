@@ -515,10 +515,12 @@ class TsdfVolume:
     DESIGN.md 4.8).  dims = (nx, ny, nz), x fastest; origin = world position of the centre of voxel (0, 0, 0);
     truncation in metres; max_weight caps a voxel's weight (one observation = 1).  intensity=True adds the
     intensity channel (8 B per voxel): keyframes then also fuse their reference image, and the surface points, mesh
-    vertices and raycast views can be shaded (surfaceIntensity, raycastIntensity)."""
+    vertices and raycast views can be shaded (surfaceIntensity, raycastIntensity).  store=True adds the brick store:
+    a shift then keeps the voxels that leave the grid and gives them back when they re-enter, and mapMesh() meshes
+    the whole map."""
 
     def __init__(self, dims, voxel_size: float, origin, truncation: float, max_weight: float = 64.0, device=-1,
-                 intensity: bool = False):
+                 intensity: bool = False, store: bool = False):
         self.dims = tuple(int(n) for n in dims)
         if len(self.dims) != 3:
             raise ValueError("TsdfVolume: dims must be (nx, ny, nz)")
@@ -533,6 +535,9 @@ class TsdfVolume:
         self.intensity = False
         if intensity:
             self.enableIntensity()
+        self.store = False
+        if store:
+            self.enableStore()
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -756,6 +761,115 @@ class TsdfVolume:
         check(self._L.rmd_volume_offset(self._h, D.ctypes.data), "TsdfVolume::offset")
         return D
 
+    def enableStore(self) -> None:
+        """Turn the brick store on (no-op when it is): from then on shift() keeps the 8x8x8 bricks of the unbounded
+        grid that leave the window with a known voxel in device memory, and restores the voxels that re-enter, so
+        that shift(d) then shift(-d) gives back the window bit for bit (DESIGN.md 4.8).  Every shift with a new
+        candidate brick then synchronises the volume's stream once."""
+        check(self._L.rmd_volume_enable_store(self._h), "TsdfVolume::enableStore")
+        self.store = True
+
+    def storeInfo(self):
+        """(stored bricks, bytes of device memory the store's pool holds)."""
+        n, b = ctypes.c_size_t(), ctypes.c_size_t()
+        check(self._L.rmd_volume_store_info(self._h, ctypes.byref(n), ctypes.byref(b)), "TsdfVolume::storeInfo")
+        return n.value, b.value
+
+    def downloadStore(self, capacity: "int | None" = None, records: bool = True):
+        """The stored bricks in ascending (z, y, x): (coords int64 [m, 3] brick coordinates (bx, by, bz), tsdf,
+        weight[, intensity, intensity weight] float32 [m, 8, 8, 8] indexed (z, y, x) like download()); voxels inside
+        the window are (0, 0).  The intensity pair comes with the channel; records=False returns the coords alone.
+        With a capacity, at most that many bricks."""
+        what = "TsdfVolume::downloadStore"
+        n = ctypes.c_size_t()
+        if capacity is None:
+            check(self._L.rmd_volume_download_store(self._h, None, None, None, None, None, 0, ctypes.byref(n)), what)
+            capacity = n.value
+        m = int(capacity)
+        coords = np.empty((m, 3), np.int64)
+        arrs = [np.empty((m, 8, 8, 8), np.float32) for _ in range((2 + 2 * self.intensity) if records else 0)]
+        ptrs = [a.ctypes.data if m else None for a in arrs] + [None] * (4 - len(arrs))
+        check(self._L.rmd_volume_download_store(self._h, coords.ctypes.data if m else None, *ptrs, m,
+                                                ctypes.byref(n)), what)
+        k = min(m, n.value)
+        if not records:
+            return coords[:k]
+        return (coords[:k],) + tuple(a[:k] for a in arrs)
+
+    def uploadStore(self, coords, tsdf, weight, intensity=None, intensity_weight=None) -> None:
+        """Replace the store with the bricks given as downloadStore() returns them (intensity pair optional: zeroed
+        colour records).  Voxels inside the window are ignored."""
+        what = "TsdfVolume::uploadStore"
+        c = np.ascontiguousarray(coords, np.int64)
+        if c.ndim != 2 or c.shape[1] != 3:
+            raise ValueError(what + ": coords must be [m, 3]")
+        m = len(c)
+        arrs = [np.ascontiguousarray(a, np.float32) for a in (tsdf, weight)]
+        if (intensity is None) != (intensity_weight is None):
+            raise ValueError(what + ": intensity and its weight come together")
+        if intensity is not None:
+            arrs += [np.ascontiguousarray(a, np.float32) for a in (intensity, intensity_weight)]
+        if any(a.size != m * 512 for a in arrs):
+            raise ValueError(what + ": records must be [m, 8, 8, 8]")
+        ptrs = [a.ctypes.data if m else None for a in arrs] + [None] * (4 - len(arrs))
+        check(self._L.rmd_volume_upload_store(self._h, c.ctypes.data if m else None, *ptrs, m), what)
+
+    def mapMesh(self, intensity: bool = False, normals: bool = False):
+        """One mesh of the whole map -- the store and the window -- as SceneMesh.mesh returns it: (float32 [n, 4]
+        vertices, int32 [m, 3] triangles, float32 [n] intensity or None, float32 [n, 3] normals or None), ready for
+        write_ply (DESIGN.md 4.8).  The window sweeps the map: tiles of its size with stride n - 1 per axis, anchored
+        at the lowest corner of the stored bricks once the window's own have been stored, so that every cube lies in
+        exactly one tile.  At each tile that meets a stored brick, in ascending (z, y, x), it takes mesh() and
+        surfaceIds(); vertices are welded by id, keeping the first tile's values.  The volume then shifts back: its
+        window, offset and store are as before, bit for bit.  Requires the store; empty when an axis has n < 2."""
+        if not self.store:
+            raise RmdError("TsdfVolume::mapMesh: the volume has no brick store", -2)
+        n = np.asarray(self.dims, np.int64)
+        D0 = self.offset
+        empty = (np.empty((0, 4), np.float32), np.empty((0, 3), np.int32),
+                 np.empty(0, np.float32) if intensity else None, np.empty((0, 3), np.float32) if normals else None)
+        if np.any(n < 2):
+            return empty
+        self.shift(n)   # every brick of the window with a known voxel goes to the store
+        bricks = self.downloadStore(records=False)
+        if not len(bricks):
+            self.shift(D0 - self.offset)
+            return empty
+        A, step = bricks.min(0) * 8, n - 1
+        # tiles t per axis whose voxels [A + t step, A + t step + n) meet a brick's [8 b, 8 b + 8)
+        lo = np.maximum(0, -((A + n - 1 - 8 * bricks) // step))
+        hi = (8 * bricks + 7 - A) // step
+        tiles = set()
+        for a, b in zip(lo, hi):
+            for tz in range(a[2], b[2] + 1):
+                for ty in range(a[1], b[1] + 1):
+                    for tx in range(a[0], b[0] + 1):
+                        tiles.add((tz, ty, tx))
+        V, T, I, N, ids, base = [], [], [], [], [], 0
+        for tz, ty, tx in sorted(tiles):
+            self.shift(A + np.array([tx, ty, tz], np.int64) * step - self.offset)
+            verts, tris = self.mesh()
+            V.append(verts)
+            T.append(tris.astype(np.int64) + base)
+            ids.append(self.surfaceIds())
+            if intensity:
+                I.append(self.surfaceIntensity())
+            if normals:
+                N.append(self.surfaceNormals())
+            base += len(verts)
+        self.shift(D0 - self.offset)
+        ids = np.concatenate(ids)
+        _, first, inv = np.unique(ids, axis=0, return_index=True, return_inverse=True)
+        order = np.argsort(first)
+        rank = np.empty(len(order), np.int64)
+        rank[order] = np.arange(len(order))
+        keep = first[order]
+        if len(keep) >= 2 ** 31:
+            raise ValueError("TsdfVolume::mapMesh: 2^31 or more vertices do not fit int32 indices")
+        tri = rank[inv.reshape(-1)][np.concatenate(T)].astype(np.int32)
+        return (np.concatenate(V)[keep], tri.reshape(-1, 3),
+                np.concatenate(I)[keep] if intensity else None, np.concatenate(N)[keep] if normals else None)
+
     def _download_records(self, fn, what: str):
         """The two halves of a record array (fn: rmd_volume_download[_intensity]), float32 of shape (nz, ny, nx)."""
         nx, ny, nz = self.dims
@@ -845,7 +959,10 @@ class SceneMesh:
     that vertex; any other vertex is new.  After a chunk, the pending ids with a voxel outside the kept box are dropped
     (that surface has left the grid, and a voxel that re-enters later starts new vertices), and the chunk's seam
     vertices become pending.  With intensity / normals, the vertices' spill-mesh and surface intensities / normals
-    are kept as well; a welded vertex keeps those of the chunk that first had it."""
+    are kept as well; a welded vertex keeps those of the chunk that first had it.
+
+    Not for a volume with the brick store: a region it revisits comes back from the store and would spill a second
+    time, so its surface would be added twice.  TsdfVolume.mapMesh meshes such a volume's whole map."""
 
     def __init__(self, intensity: bool = False, normals: bool = False):
         self.intensity, self.normals = bool(intensity), bool(normals)

@@ -894,6 +894,70 @@ __global__ void __launch_bounds__(256) volume_prior_kernel(const VolumeRaycastPa
   S.seed[(size_t)y * S.seed_stride + x] = make_float4(d, S.sigma_sq, 10.0f, 10.0f);
 }
 
+// ------------------------------------------------------------------------------------------------- brick store
+// One CTA per brick, one thread per brick voxel (x fastest): the window index of voxel l of brick q, or -1 when the
+// voxel does not move (DESIGN.md 4.8).  A candidate brick lies within 8 voxels of the window, so that 8 b - W fits.
+__device__ __forceinline__ long long store_moving_voxel(const VolumeStoreParams &P, const VolumeStoreBrick &B, int l)
+{
+  const int n[3] = {P.g.nx, P.g.ny, P.g.nz};
+  const int loc[3] = {l & 7, (l >> 3) & 7, l >> 6};
+  int w[3];
+  bool inside = true;
+  for(int a = 0; a < 3; ++a)
+  {
+    w[a] = (int)(B.b[a] * 8 - P.W[a]) + loc[a];
+    if(w[a] < 0 || w[a] >= n[a])
+      return -1;
+    inside = inside && w[a] >= P.lo[a] && w[a] < P.hi[a];
+  }
+  if(inside)
+    return -1;
+  return ((long long)w[2] * P.g.ny + w[1]) * P.g.nx + w[0];
+}
+
+__global__ void __launch_bounds__(512) volume_store_flag_kernel(const VolumeStoreParams P)
+{
+  const VolumeStoreBrick B = P.bricks[blockIdx.x];
+  const long long w = store_moving_voxel(P, B, threadIdx.x);
+  const int seen = w >= 0 && P.g.vox[w].y > 0.0f;
+  const int any = __syncthreads_or(seen);
+  if(threadIdx.x == 0)
+    P.flags[blockIdx.x] = any;
+}
+
+template<bool INTENSITY>
+__global__ void __launch_bounds__(512) volume_store_evict_kernel(const VolumeStoreParams P)
+{
+  const VolumeStoreBrick B = P.bricks[blockIdx.x];
+  const long long w = store_moving_voxel(P, B, threadIdx.x);
+  const size_t dst = (size_t)B.slot * VOLUME_STORE_VOXELS + threadIdx.x;
+  if(w >= 0)
+  {
+    P.pool[dst] = P.g.vox[w];
+    if(INTENSITY)
+      P.pool_col[dst] = P.col[w];
+  }
+  else if(B.fresh)
+  {
+    P.pool[dst] = make_float2(0.0f, 0.0f);
+    if(INTENSITY)
+      P.pool_col[dst] = make_float2(0.0f, 0.0f);
+  }
+}
+
+template<bool INTENSITY>
+__global__ void __launch_bounds__(512) volume_store_restore_kernel(const VolumeStoreParams P)
+{
+  const VolumeStoreBrick B = P.bricks[blockIdx.x];
+  const long long w = store_moving_voxel(P, B, threadIdx.x);
+  if(w < 0)
+    return;
+  const size_t src = (size_t)B.slot * VOLUME_STORE_VOXELS + threadIdx.x;
+  P.g.vox[w] = P.pool[src];
+  if(INTENSITY)
+    P.col[w] = P.pool_col[src];
+}
+
 } // namespace
 
 cudaError_t launch_volume_integrate(const VolumeIntegrateParams &P, cudaStream_t stream)
@@ -1033,6 +1097,31 @@ cudaError_t launch_volume_spill_tri_count(const VolumeMeshParams &P, const Volum
 cudaError_t launch_volume_spill_tri_write(const VolumeMeshParams &P, const VolumeSpillBox &K, cudaStream_t stream)
 {
   volume_spill_tri_write_kernel<<<P.b.n_blocks, VOLUME_SURF_BLOCK, 0, stream>>>(P, K);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_store_flag(const VolumeStoreParams &P, unsigned int n, cudaStream_t stream)
+{
+  if(n)
+    volume_store_flag_kernel<<<n, VOLUME_STORE_VOXELS, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_store_evict(const VolumeStoreParams &P, unsigned int n, cudaStream_t stream)
+{
+  if(n && P.col)
+    volume_store_evict_kernel<true><<<n, VOLUME_STORE_VOXELS, 0, stream>>>(P);
+  else if(n)
+    volume_store_evict_kernel<false><<<n, VOLUME_STORE_VOXELS, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_store_restore(const VolumeStoreParams &P, unsigned int n, cudaStream_t stream)
+{
+  if(n && P.col)
+    volume_store_restore_kernel<true><<<n, VOLUME_STORE_VOXELS, 0, stream>>>(P);
+  else if(n)
+    volume_store_restore_kernel<false><<<n, VOLUME_STORE_VOXELS, 0, stream>>>(P);
   return cudaGetLastError();
 }
 

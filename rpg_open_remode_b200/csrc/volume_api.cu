@@ -7,12 +7,27 @@
 
 #include <new>
 #include <string>
+#include <vector>
 
 #include "rmd_common.cuh"
 #include "volume.cuh"
+#include "volume_store.h"
 
 namespace rmdb
 {
+
+static_assert(STORE_BRICK_VOXELS == VOLUME_STORE_VOXELS, "one brick size on host and device");
+
+// The brick store (DESIGN.md 4.8): the host index, the device pool of cap bricks (pool_col with the intensity
+// channel) and the per-shift scratch: the bricks the kernels visit and the flag kernel's flags.
+struct VolumeStore
+{
+  BrickIndex index;
+  float2 *pool, *pool_col;
+  size_t cap;
+  VolumeStoreBrick *bricks; size_t bricks_cap;
+  int *flags; size_t flags_cap;
+};
 
 int volume_integrate(rmd_volume *v, VolumeIntegrateParams &P)
 {
@@ -448,6 +463,160 @@ int volume_spill_mesh(rmd_volume *v, const VolumeSpillBox &K, float *xyzw, size_
   return 0;
 }
 
+int no_store(const char *what)
+{
+  return fail(RMD_ERR_NOT_INITIALISED, (std::string(what) + ": the volume has no brick store").c_str());
+}
+
+// The store's pool grown to hold `need` bricks, by doubling: the new arrays of both channels are allocated before the
+// used slots are copied and the old arrays freed, so that a failure leaves the store as it was.
+int store_grow(rmd_volume *v, size_t need, const char *what)
+{
+  VolumeStore *S = v->store;
+  const size_t cap = store_pool_capacity(S->cap, need);
+  if(cap == S->cap)
+    return 0;
+  const size_t brick = sizeof(float2) * VOLUME_STORE_VOXELS, used = brick * S->index.slot.size();
+  float2 *p = NULL, *pc = NULL;
+  cudaError_t err = cudaMalloc(&p, brick * cap);
+  if(err == cudaSuccess && v->col) err = cudaMalloc(&pc, brick * cap);
+  if(err == cudaSuccess && used) err = cudaMemcpyAsync(p, S->pool, used, cudaMemcpyDeviceToDevice, v->stream);
+  if(err == cudaSuccess && used && v->col)
+    err = cudaMemcpyAsync(pc, S->pool_col, used, cudaMemcpyDeviceToDevice, v->stream);
+  if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);
+  if(err != cudaSuccess)
+  {
+    cudaFree(p); cudaFree(pc);
+    return fail_cuda(err, what);
+  }
+  cudaFree(S->pool); cudaFree(S->pool_col);
+  S->pool = p; S->pool_col = pc; S->cap = cap;
+  return 0;
+}
+
+// The bricks a store kernel visits, to the device (scratch grown by the caller).  Pageable source: the copy is staged
+// before the call returns.
+int store_upload_bricks(rmd_volume *v, const std::vector<VolumeStoreBrick> &list)
+{
+  if(!list.empty())
+    RMD_CUDA_TRY(cudaMemcpyAsync(v->store->bricks, list.data(), sizeof(VolumeStoreBrick) * list.size(),
+                                 cudaMemcpyHostToDevice, v->stream));
+  return 0;
+}
+
+VolumeStoreBrick store_brick(const BrickCoord &c, int slot, int fresh)
+{
+  VolumeStoreBrick B;
+  B.b[0] = c.b[0]; B.b[1] = c.b[1]; B.b[2] = c.b[2];
+  B.slot = slot; B.fresh = fresh;
+  return B;
+}
+
+// The store's part of rmd_volume_shift before the gather (DESIGN.md 4.8): the candidates -- bricks with a voxel that
+// leaves -- split into stored and fresh; the fresh ones flagged on the device and the flags read back (the shift's one
+// host synchronisation); the pool and scratch grown; then, the first write, the index updated and the evict kernel
+// launched on the pre-shift records.  The stored bricks with a voxel that enters follow the evicted ones in the
+// scratch, from *restore_first on, *n_restore of them, for store_restore after the gather.
+int store_evict(rmd_volume *v, const int d[3], const long long Dnew[3], size_t *restore_first, size_t *n_restore)
+{
+  const char *what = "rmd_volume_shift";
+  VolumeStore *S = v->store;
+  const int n[3] = {v->g.nx, v->g.ny, v->g.nz};
+  const VolumeSpillBox K = spill_box(v, d);
+  VolumeSpillBox Kin;   // post-shift indices whose source lay in the grid
+  for(int a = 0; a < 3; ++a)
+  {
+    const int c = d[a] < -n[a] ? -n[a] : d[a] > n[a] ? n[a] : d[a];
+    Kin.lo[a] = c < 0 ? -c : 0;
+    Kin.hi[a] = c > 0 ? n[a] - c : n[a];
+  }
+  const int64_t Dold[3] = {v->D[0], v->D[1], v->D[2]}, Dn[3] = {Dnew[0], Dnew[1], Dnew[2]};
+  std::vector<BrickCoord> known, fresh;
+  S->index.split(store_candidates(Dold, n, K.lo, K.hi), known, fresh);
+  const std::vector<BrickCoord> entering = store_candidates(Dn, n, Kin.lo, Kin.hi);
+
+  VolumeStoreParams P;
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.col = v->col;
+  for(int a = 0; a < 3; ++a)
+  {
+    P.W[a] = Dold[a];
+    P.lo[a] = K.lo[a]; P.hi[a] = K.hi[a];
+  }
+  int rc = volume_grow(&S->bricks, &S->bricks_cap, known.size() + fresh.size() + entering.size());
+  if(!rc) rc = volume_grow(&S->flags, &S->flags_cap, fresh.size());
+  if(rc) return rc;
+  P.bricks = S->bricks;
+  P.flags = S->flags;
+  std::vector<int> flags(fresh.size(), 0);
+  std::vector<VolumeStoreBrick> list;
+  if(!fresh.empty())
+  {
+    for(size_t q = 0; q < fresh.size(); ++q)
+      list.push_back(store_brick(fresh[q], (int)q, 1));
+    rc = store_upload_bricks(v, list);
+    if(rc) return rc;
+    RMD_CUDA_TRY(launch_volume_store_flag(P, (unsigned int)fresh.size(), v->stream));
+    RMD_CUDA_TRY(cudaMemcpyAsync(flags.data(), S->flags, sizeof(int) * fresh.size(), cudaMemcpyDeviceToHost,
+                                 v->stream));
+    RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  }
+  size_t added = 0;
+  for(int f : flags)
+    added += f ? 1 : 0;
+  if(S->index.slot.size() + added > (size_t)INT32_MAX)
+    return fail(RMD_ERR_UNSUPPORTED, "rmd_volume_shift: 2^31 or more stored bricks");
+  rc = store_grow(v, S->index.slot.size() + added, what);
+  if(rc) return rc;
+
+  // nothing has been written so far; from here on the shift happens
+  const std::vector<BrickCoord> added_bricks = S->index.add(fresh, flags);
+  list.clear();
+  for(const BrickCoord &c : known)
+    list.push_back(store_brick(c, S->index.slot.at(c), 0));
+  for(const BrickCoord &c : added_bricks)
+    list.push_back(store_brick(c, S->index.slot.at(c), 1));
+  const size_t n_evict = list.size();
+  for(const BrickCoord &c : entering)
+  {
+    auto it = S->index.slot.find(c);
+    if(it != S->index.slot.end())
+      list.push_back(store_brick(c, it->second, 0));
+  }
+  *restore_first = n_evict;
+  *n_restore = list.size() - n_evict;
+  rc = store_upload_bricks(v, list);
+  if(rc) return rc;
+  P.pool = S->pool; P.pool_col = S->pool_col;
+  RMD_CUDA_TRY(launch_volume_store_evict(P, (unsigned int)n_evict, v->stream));
+  return 0;
+}
+
+// The store's part of rmd_volume_shift after the gather: the stored bricks' entering voxels into the new records.
+int store_restore(rmd_volume *v, const int d[3], size_t first, size_t count)
+{
+  if(!count)
+    return 0;
+  VolumeStore *S = v->store;
+  const int n[3] = {v->g.nx, v->g.ny, v->g.nz};
+  VolumeStoreParams P;
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.col = v->col;
+  P.pool = S->pool; P.pool_col = S->pool_col;
+  P.bricks = S->bricks + first;
+  for(int a = 0; a < 3; ++a)
+  {
+    const int c = d[a] < -n[a] ? -n[a] : d[a] > n[a] ? n[a] : d[a];
+    P.W[a] = v->D[a];
+    P.lo[a] = c < 0 ? -c : 0;
+    P.hi[a] = c > 0 ? n[a] - c : n[a];
+  }
+  RMD_CUDA_TRY(launch_volume_store_restore(P, (unsigned int)count, v->stream));
+  return 0;
+}
+
 // origin + (float)D * s, one rounding per operation as the kernels' voxel_coord (volatile: no contraction)
 float shifted_origin(float origin, long long D, float s)
 {
@@ -513,6 +682,12 @@ int rmd_volume_destroy(rmd_volume_t *v)
   cudaFree(v->tri_offsets); cudaFree(v->tri_total); cudaFree(v->keys); cudaFree(v->tri_stage);
   cudaFree(v->col);
   cudaFree(v->vox_alt); cudaFree(v->col_alt);
+  if(v->store)
+  {
+    cudaFree(v->store->pool); cudaFree(v->store->pool_col);
+    cudaFree(v->store->bricks); cudaFree(v->store->flags);
+    delete v->store;
+  }
   cudaGetLastError();
   delete v;
   return 0;
@@ -534,6 +709,8 @@ int rmd_volume_reset(rmd_volume_t *v)
   RMD_CUDA_TRY(cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->stream));
   if(v->col)
     RMD_CUDA_TRY(cudaMemsetAsync(v->col, 0, sizeof(float2) * v->n_vox, v->stream));
+  if(v->store)
+    v->store->index.slot.clear();
   return 0;
 }
 
@@ -571,8 +748,24 @@ int rmd_volume_shift(rmd_volume_t *v, const int d[3])
     o[a] = shifted_origin(v->o0[a], D[a], v->g.voxel);
     RMD_REQUIRE(isfinite(o[a]), "rmd_volume_shift: the origin would not be finite");
     gather = gather && (d[a] < 0 ? -(long long)d[a] : (long long)d[a]) < n[a];
+    long long end;
+    RMD_REQUIRE(!v->store || !__builtin_add_overflow(D[a], (long long)n[a], &end),
+                "rmd_volume_shift: the total offset plus the grid size overflows");
   }
   DeviceGuard guard(v->device);
+  if(gather)
+  {
+    if(!v->vox_alt)
+      RMD_CUDA_TRY(cudaMalloc(&v->vox_alt, sizeof(float2) * v->n_vox));
+    if(v->col && !v->col_alt)
+      RMD_CUDA_TRY(cudaMalloc(&v->col_alt, sizeof(float2) * v->n_vox));
+  }
+  size_t restore_first = 0, n_restore = 0;
+  if(v->store)
+  {
+    const int rc = store_evict(v, d, D, &restore_first, &n_restore);
+    if(rc) return rc;
+  }
   if(!gather)   // nothing stays in the grid
   {
     RMD_CUDA_TRY(cudaMemsetAsync(v->g.vox, 0, sizeof(float2) * v->n_vox, v->stream));
@@ -581,10 +774,6 @@ int rmd_volume_shift(rmd_volume_t *v, const int d[3])
   }
   else
   {
-    if(!v->vox_alt)
-      RMD_CUDA_TRY(cudaMalloc(&v->vox_alt, sizeof(float2) * v->n_vox));
-    if(v->col && !v->col_alt)
-      RMD_CUDA_TRY(cudaMalloc(&v->col_alt, sizeof(float2) * v->n_vox));
     VolumeShiftParams P;
     memset(&P, 0, sizeof(P));
     P.g = v->g;
@@ -606,6 +795,8 @@ int rmd_volume_shift(rmd_volume_t *v, const int d[3])
   for(int a = 0; a < 3; ++a)
     v->D[a] = D[a];
   v->g.ox = o[0]; v->g.oy = o[1]; v->g.oz = o[2];
+  if(v->store)
+    return store_restore(v, d, restore_first, n_restore);
   return 0;
 }
 
@@ -703,6 +894,18 @@ int rmd_volume_enable_intensity(rmd_volume_t *v)
     return fail_cuda(err, "rmd_volume_enable_intensity");
   }
   err = cudaMemsetAsync(v->col, 0, sizeof(float2) * v->n_vox, v->stream);
+  VolumeStore *S = v->store;
+  const size_t pool_bytes = S ? sizeof(float2) * VOLUME_STORE_VOXELS * S->cap : 0;
+  if(err == cudaSuccess && pool_bytes)   // the bricks already stored get zeroed colour records
+  {
+    err = cudaMalloc(&S->pool_col, pool_bytes);
+    if(err == cudaSuccess) err = cudaMemsetAsync(S->pool_col, 0, pool_bytes, v->stream);
+    if(err != cudaSuccess)
+    {
+      cudaFree(S->pool_col);
+      S->pool_col = NULL;
+    }
+  }
   if(err != cudaSuccess)
   {
     cudaFree(v->col);
@@ -854,6 +1057,134 @@ int rmd_volume_upload_intensity(rmd_volume_t *v, const float *host_intensity, co
     return no_intensity("rmd_volume_upload_intensity");
   DeviceGuard guard(v->device);
   return volume_upload_records(v, v->col, host_intensity, host_weight, "rmd_volume_upload_intensity");
+}
+
+int rmd_volume_enable_store(rmd_volume_t *v)
+{
+  const char *what = "rmd_volume_enable_store";
+  VOLUME_REQUIRE(v, "null handle");
+  if(v->store)
+    return 0;
+  const int n[3] = {v->g.nx, v->g.ny, v->g.nz};
+  for(int a = 0; a < 3; ++a)
+  {
+    long long end;
+    VOLUME_REQUIRE(!__builtin_add_overflow(v->D[a], (long long)n[a], &end),
+                   "the total offset plus the grid size overflows");
+  }
+  v->store = new(std::nothrow) VolumeStore();
+  if(!v->store)
+    return fail((int)cudaErrorMemoryAllocation, "rmd_volume_enable_store: host allocation failed");
+  return 0;
+}
+
+int rmd_volume_store_info(rmd_volume_t *v, size_t *bricks, size_t *bytes)
+{
+  const char *what = "rmd_volume_store_info";
+  VOLUME_REQUIRE(v, "null handle");
+  if(!v->store)
+    return no_store(what);
+  if(bricks) *bricks = v->store->index.slot.size();
+  if(bytes) *bytes = sizeof(float2) * VOLUME_STORE_VOXELS * v->store->cap * (v->store->pool_col ? 2 : 1);
+  return 0;
+}
+
+int rmd_volume_download_store(rmd_volume_t *v, int64_t *host_coords, float *host_tsdf, float *host_weight,
+                              float *host_intensity, float *host_intensity_weight, size_t capacity, size_t *count)
+{
+  const char *what = "rmd_volume_download_store";
+  VOLUME_REQUIRE(v && count && (host_coords || capacity == 0), "null argument");
+  if((host_intensity || host_intensity_weight) && !v->col)
+    return no_intensity(what);
+  if(!v->store)
+    return no_store(what);
+  DeviceGuard guard(v->device);
+  VolumeStore *S = v->store;
+  *count = S->index.slot.size();
+  const size_t m = *count < capacity ? *count : capacity;
+  if(!m)
+    return 0;
+  const bool records = host_tsdf || host_weight, colour = host_intensity || host_intensity_weight;
+  const size_t used = VOLUME_STORE_VOXELS * S->index.slot.size();
+  std::vector<float2> rec(records ? used : 0), col(colour ? used : 0);
+  // the store's copies of voxels that are in the window are stale: wait for the window's last writes, then read
+  if(records)
+    RMD_CUDA_TRY(cudaMemcpyAsync(rec.data(), S->pool, sizeof(float2) * used, cudaMemcpyDeviceToHost, v->stream));
+  if(colour)
+    RMD_CUDA_TRY(cudaMemcpyAsync(col.data(), S->pool_col, sizeof(float2) * used, cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  const int n[3] = {v->g.nx, v->g.ny, v->g.nz};
+  size_t q = 0;
+  for(auto it = S->index.slot.begin(); it != S->index.slot.end() && q < m; ++it, ++q)
+  {
+    const BrickCoord &c = it->first;
+    for(int a = 0; a < 3; ++a)
+      host_coords[3 * q + a] = c.b[a];
+    for(int l = 0; l < VOLUME_STORE_VOXELS; ++l)
+    {
+      const int loc[3] = {l & 7, (l >> 3) & 7, l >> 6};
+      bool in_window = true;
+      for(int a = 0; a < 3; ++a)
+      {
+        const int64_t u = c.b[a] * STORE_BRICK + loc[a];
+        in_window = in_window && u >= v->D[a] && (uint64_t)u - (uint64_t)v->D[a] < (uint64_t)n[a];
+      }
+      const size_t src = (size_t)it->second * VOLUME_STORE_VOXELS + l, dst = q * VOLUME_STORE_VOXELS + l;
+      const float2 zero = make_float2(0.0f, 0.0f);
+      const float2 r = in_window || !records ? zero : rec[src], k = in_window || !colour ? zero : col[src];
+      if(host_tsdf) host_tsdf[dst] = r.x;
+      if(host_weight) host_weight[dst] = r.y;
+      if(host_intensity) host_intensity[dst] = k.x;
+      if(host_intensity_weight) host_intensity_weight[dst] = k.y;
+    }
+  }
+  return 0;
+}
+
+int rmd_volume_upload_store(rmd_volume_t *v, const int64_t *host_coords, const float *host_tsdf,
+                            const float *host_weight, const float *host_intensity,
+                            const float *host_intensity_weight, size_t count)
+{
+  const char *what = "rmd_volume_upload_store";
+  VOLUME_REQUIRE(v && (count == 0 || (host_coords && host_tsdf && host_weight)), "null argument");
+  VOLUME_REQUIRE(!host_intensity == !host_intensity_weight, "intensity and its weight come together");
+  if(host_intensity && !v->col)
+    return no_intensity(what);
+  if(!v->store)
+    return no_store(what);
+  VOLUME_REQUIRE(count <= (size_t)INT32_MAX, "2^31 or more bricks");
+  BrickIndex index;
+  const int64_t bmin = INT64_MIN / STORE_BRICK, bmax = INT64_MAX / STORE_BRICK;   // 8 b + 7 fits
+  for(size_t q = 0; q < count; ++q)
+  {
+    BrickCoord c;
+    for(int a = 0; a < 3; ++a)
+    {
+      c.b[a] = host_coords[3 * q + a];
+      VOLUME_REQUIRE(c.b[a] >= bmin && c.b[a] <= bmax, "brick coordinate out of range");
+    }
+    VOLUME_REQUIRE(index.slot.emplace(c, (int)q).second, "duplicate brick");
+  }
+  DeviceGuard guard(v->device);
+  int rc = store_grow(v, count, what);
+  if(rc) return rc;
+  const size_t used = VOLUME_STORE_VOXELS * count;
+  std::vector<float2> rec(used);
+  for(size_t i = 0; i < used; ++i)
+    rec[i] = make_float2(host_tsdf[i], host_weight[i]);
+  if(used)
+    RMD_CUDA_TRY(cudaMemcpyAsync(v->store->pool, rec.data(), sizeof(float2) * used, cudaMemcpyHostToDevice,
+                                 v->stream));
+  if(used && v->col)
+  {
+    for(size_t i = 0; i < used; ++i)
+      rec[i] = host_intensity ? make_float2(host_intensity[i], host_intensity_weight[i]) : make_float2(0.0f, 0.0f);
+    RMD_CUDA_TRY(cudaMemcpyAsync(v->store->pool_col, rec.data(), sizeof(float2) * used, cudaMemcpyHostToDevice,
+                                 v->stream));
+  }
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  v->store->index.slot.swap(index.slot);
+  return 0;
 }
 
 } // extern "C"

@@ -38,6 +38,9 @@ class DepthmapNode:
             raise ValueError("DepthmapNode: follow_volume needs a volume")
         if scene_mesh is not None and not follow_volume:
             raise ValueError("DepthmapNode: scene_mesh needs follow_volume=True")
+        if scene_mesh is not None and getattr(volume, "store", False):
+            raise ValueError("DepthmapNode: scene_mesh would add a revisited region of a volume with the brick store "
+                             "twice; mesh its map with volume.mapMesh()")
         if not 0.0 <= prior_from_volume <= 1.0:
             raise ValueError("DepthmapNode: prior_from_volume must be in [0, 1] (0 = off)")
         self.depthmap_ = depthmap
