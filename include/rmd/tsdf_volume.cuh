@@ -249,6 +249,24 @@ public:
                            "TsdfVolume: unable to upload the store");
   }
 
+  // Euclidean signed distance field of the current window: per voxel the distance (metres) to the nearest occupied
+  // voxel (weight > 0, tsdf <= 0) for the others, minus that to the nearest other voxel for an occupied one; +-inf
+  // when one set is empty.  Asynchronous; the snapshot and its origin stay until the next computeEsdf().  The first
+  // call allocates 16 B per voxel.  Throws past (nx-1)^2 + (ny-1)^2 + (nz-1)^2 >= 2^24.
+  void computeEsdf() { detail::throw_on_error(rmd_volume_esdf(handle_), "TsdfVolume: unable to compute the ESDF"); }
+  // The snapshot's distance and weight, nx * ny * nz floats each.
+  void downloadEsdf(float *host_distance, float *host_weight)
+  {
+    detail::throw_on_error(rmd_volume_download_esdf(handle_, host_distance, host_weight),
+                           "TsdfVolume: unable to download the ESDF");
+  }
+  // At n world points (4 floats each, w ignored): 4 floats (distance, d/dx, d/dy, d/dz) per point to dg and the min
+  // corner weight to weight (NULL: not wanted); outside the grid (NaN, 0, 0, 0) and weight 0.  Synchronous.
+  void esdfQuery(const float *xyzw, size_t n, float *dg, float *weight = NULL)
+  {
+    detail::throw_on_error(rmd_volume_esdf_query(handle_, xyzw, n, dg, weight), "TsdfVolume: unable to query the ESDF");
+  }
+
   void downloadIntensity(float *host_intensity, float *host_weight)
   {
     detail::throw_on_error(rmd_volume_download_intensity(handle_, host_intensity, host_weight),

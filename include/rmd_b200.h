@@ -759,6 +759,52 @@ int rmd_volume_upload_store(rmd_volume_t *v, const int64_t *host_coords, const f
                             const float *host_weight, const float *host_intensity,
                             const float *host_intensity_weight, size_t count);
 
+/* Euclidean signed distance field (DESIGN.md 4.8): how far a point is from
+ * the nearest obstacle of the current window, and in which direction.
+ *   O (occupied) = the voxels with weight > 0 && tsdf <= 0 (float compares:
+ * -0.0 is occupied, a NaN tsdf is not); F = every other voxel, unknown ones
+ * included.  d2_X(v) = min over u in X of |v - u|^2 with integer voxel
+ * indices: exact, and unique.  rmd_volume_esdf computes the snapshot, one
+ * (distance, weight) per voxel, indexed like the records: distance =
+ * s * sqrt(d2_O(v)) for v in F and -s * sqrt(d2_F(v)) for v in O (fp32:
+ * __fmul_rn(__fsqrt_rn((float)d2), s)), +inf everywhere when O is empty and
+ * -inf when F is empty; weight = the record's weight, bit for bit, at the
+ * time of the call (0 = unknown).  Obstacles in the brick store or outside the
+ * window are not seen, so near the window's faces a distance is an upper
+ * bound.  Requires (nx-1)^2 + (ny-1)^2 + (nz-1)^2 < 2^24 (every squared
+ * distance exact in fp32): RMD_ERR_UNSUPPORTED otherwise.
+ *   Memory: 16 B per voxel -- the 8 B snapshot and 8 B of scratch --
+ * allocated by the first compute (cudaErrorMemoryAllocation when it does not
+ * fit) and freed by rmd_volume_destroy; 2 GiB at 512^3.  A volume that never
+ * computes an ESDF allocates nothing.
+ *   Only a compute writes the snapshot: later integrations, shifts, uploads
+ * and resets leave it and its origin as they were, so queries answer for the
+ * window as it was at the compute.  All calls are ordered on the volume's
+ * stream; rmd_volume_esdf and rmd_volume_esdf_query_device are asynchronous,
+ * the host variants synchronous.
+ *   Query at world point p = (x, y, z) of each float4 (w ignored, so
+ * rmd_volume_surface_points output can be queried as it is): grid
+ * coordinates u = (p - origin) / s per axis (round to nearest), the cell of
+ * the raycast's trilinear sample (floor, corner i0 and i0 + 1 inside the
+ * grid).  Outside (no such cell, or p not finite): (NaN, 0, 0, 0), weight 0.
+ * Otherwise weight = the min of the 8 corner weights (0: the cell touches
+ * unknown space) and, when a corner's distance is infinite, the distance is
+ * the first such corner's (x fastest) and the gradient (0, 0, 0); else the
+ * distance is trilinear in x, then y, then z, and the gradient the analytic
+ * derivative of that trilinear function in metres.  Output: one float4
+ * (distance, d/dx, d/dy, d/dz) per point to dg, one float per point to the
+ * weights (may be NULL).  The device variant wants 16-byte aligned points and
+ * outputs.
+ *   RMD_ERR_NOT_INITIALISED: a query or download before the first compute.
+ * RMD_ERR_INVALID_ARGUMENT: null handle or pointer (n = 0 allows NULL
+ * points and outputs), misaligned device pointers. */
+int rmd_volume_esdf(rmd_volume_t *v);
+/* Test / checkpoint hook (like rmd_volume_download): the snapshot's distance
+ * and weight, nx * ny * nz floats each.  Synchronous. */
+int rmd_volume_download_esdf(rmd_volume_t *v, float *host_distance, float *host_weight);
+int rmd_volume_esdf_query(rmd_volume_t *v, const float *host_xyzw, size_t n, float *host_dg, float *host_weight);
+int rmd_volume_esdf_query_device(rmd_volume_t *v, const float *dev_xyzw, size_t n, float *dev_dg, float *dev_weight);
+
 /* ---------------------------------------------------------- device image */
 
 /* DeviceImage<T>(width,height) = cudaMallocPitch, device_image.cuh:37-50 */

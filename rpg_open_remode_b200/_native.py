@@ -110,6 +110,10 @@ _SIGNATURES = {
     "rmd_volume_store_info": (ci, [vp, P(cs), P(cs)]),
     "rmd_volume_download_store": (ci, [vp, vp, vp, vp, vp, vp, cs, P(cs)]),
     "rmd_volume_upload_store": (ci, [vp, vp, vp, vp, vp, vp, cs]),
+    "rmd_volume_esdf": (ci, [vp]),
+    "rmd_volume_download_esdf": (ci, [vp, vp, vp]),
+    "rmd_volume_esdf_query": (ci, [vp, vp, cs, vp, vp]),
+    "rmd_volume_esdf_query_device": (ci, [vp, vp, cs, vp, vp]),
     "rmd_reduce_sum_f32":(ci, [vp, cs, cs, cs, P(cf)]),
     "rmd_reduce_sum_i32": (ci, [vp, cs, cs, cs, P(ctypes.c_int32)]),
     "rmd_reduce_count_eq_i32": (ci, [vp, cs, cs, cs, ctypes.c_int32, P(cs)]),

@@ -870,6 +870,43 @@ class TsdfVolume:
         return (np.concatenate(V)[keep], tri.reshape(-1, 3),
                 np.concatenate(I)[keep] if intensity else None, np.concatenate(N)[keep] if normals else None)
 
+    def computeEsdf(self) -> None:
+        """Compute the Euclidean signed distance field of the current window (DESIGN.md 4.8): per voxel the distance
+        in metres to the nearest occupied voxel (weight > 0 and tsdf <= 0) for a free or unknown voxel, minus the
+        distance to the nearest other voxel for an occupied one; +inf / -inf everywhere when no voxel is occupied /
+        free.  Obstacles outside the window are not seen.  Asynchronous on the volume's stream; the snapshot and its
+        origin stay as they are until the next computeEsdf(), whatever the volume does meanwhile.  The first call
+        allocates 16 B per voxel.  Raises RmdError (RMD_ERR_UNSUPPORTED) unless (nx-1)^2 + (ny-1)^2 + (nz-1)^2 < 2^24."""
+        check(self._L.rmd_volume_esdf(self._h), "TsdfVolume::computeEsdf")
+
+    def downloadEsdf(self):
+        """(distance, weight) of the snapshot, float32 arrays of shape (nz, ny, nx); weight = the records' weight at
+        the compute (0 = unknown)."""
+        return self._download_records(self._L.rmd_volume_download_esdf, "TsdfVolume::downloadEsdf")
+
+    def esdfQuery(self, points):
+        """(dg float32 [N, 4] = (distance, d/dx, d/dy, d/dz), weight float32 [N]) at world points [N, 3] or [N, 4]
+        (w ignored, so surfacePoints() can be queried as it is): the snapshot trilinear at each point and its
+        gradient in metres; weight = the min of the cell's 8 corner weights.  Outside the window: distance NaN,
+        gradient 0, weight 0."""
+        p = np.asarray(points, np.float32)
+        if p.ndim != 2 or p.shape[1] not in (3, 4):
+            raise ValueError("TsdfVolume::esdfQuery: points must be [N, 3] or [N, 4]")
+        xyzw = np.zeros((len(p), 4), np.float32)
+        xyzw[:, :p.shape[1]] = p
+        dg, w = np.empty((len(p), 4), np.float32), np.empty(len(p), np.float32)
+        n = len(p)
+        check(self._L.rmd_volume_esdf_query(self._h, xyzw.ctypes.data if n else None, n,
+                                            dg.ctypes.data if n else None, w.ctypes.data if n else None),
+              "TsdfVolume::esdfQuery")
+        return dg, w
+
+    def esdfQueryDevice(self, dev_xyzw: int, n: int, dev_dg: int, dev_weight: "int | None" = None) -> None:
+        """esdfQuery on device memory: n float4 points at dev_xyzw, n float4 (distance, gradient) to dev_dg and,
+        when given, n float weights to dev_weight.  Asynchronous on the volume's stream."""
+        check(self._L.rmd_volume_esdf_query_device(self._h, dev_xyzw, int(n), dev_dg, dev_weight),
+              "TsdfVolume::esdfQueryDevice")
+
     def _download_records(self, fn, what: str):
         """The two halves of a record array (fn: rmd_volume_download[_intensity]), float32 of shape (nz, ny, nx)."""
         nx, ny, nz = self.dims

@@ -958,6 +958,182 @@ __global__ void __launch_bounds__(512) volume_store_restore_kernel(const VolumeS
     P.col[w] = P.pool_col[src];
 }
 
+// -------------------------------------------------------------------------------------------------------- ESDF
+// The packed value of voxel idx at the start of pass PASS: the z pass reads the record (the distance to the other set
+// is not known yet), the others the previous pass's output.
+template<int PASS>
+__device__ __forceinline__ int esdf_in(const VolumeEsdfParams &P, size_t idx)
+{
+  if(PASS == 0)
+  {
+    const float2 r = __ldg(P.g.vox + idx);
+    return (r.y > 0.0f && r.x <= 0.0f) ? (int)(0x80000000u | (unsigned int)ESDF_INF) : ESDF_INF;
+  }
+  return __ldg(P.in + idx);
+}
+
+// The parabola height of a packed value for set s (0 = O, 1 = F): 0 on the set's own voxels, else the squared distance
+// to the set so far (ESDF_INF: not a site).
+__device__ __forceinline__ int esdf_site(int packed, int s)
+{
+  return ((packed < 0) == (s == 0)) ? 0 : (packed & ESDF_INF);
+}
+
+// One thread per column of the pass's axis (z: columns (i, j); y: (i, k); x: (j, k)), 32 adjacent columns per warp.
+// Phase 1 builds both sets' lower envelopes in one sweep; phase 2 sweeps again and evaluates, at each voxel, the
+// envelope of the set it does not belong to.  Each envelope keeps its top two (phase 1) or current and next (phase 2)
+// entries in registers; F = f + p^2 in int64.
+template<int PASS>
+__global__ void __launch_bounds__(256) volume_esdf_kernel(const VolumeEsdfParams P)
+{
+  const VolumeGrid &g = P.g;
+  const size_t plane = (size_t)g.nx * (size_t)g.ny;
+  const size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  size_t ncol, base, stride;
+  int n;
+  if(PASS == 0)      { ncol = plane; base = c; stride = plane; n = g.nz; }
+  else if(PASS == 1) { ncol = (size_t)g.nx * g.nz; base = (c / g.nx) * plane + c % g.nx; stride = g.nx; n = g.ny; }
+  else               { ncol = (size_t)g.ny * g.nz; base = c * g.nx; stride = 1; n = g.nx; }
+  if(c >= ncol)
+    return;
+  const size_t n_vox = plane * (size_t)g.nz;
+  unsigned short *stack[2] = {P.stack + base, P.stack + n_vox + base};   // entry e at [e * stride]
+
+  // phase 1: the envelopes; (va, Fa) below the top, (vb, Fb) the top
+  int top[2] = {-1, -1}, va[2] = {0, 0}, vb[2] = {0, 0};
+  long long Fa[2] = {0, 0}, Fb[2] = {0, 0};
+  for(int q = 0; q < n; ++q)
+  {
+    const int p = esdf_in<PASS>(P, base + (size_t)q * stride);
+#pragma unroll
+    for(int s = 0; s < 2; ++s)
+    {
+      const int f = esdf_site(p, s);
+      if(f == ESDF_INF)
+        continue;
+      const long long Fq = (long long)f + (long long)q * q;
+      // pop the top b while the new parabola's intersection with it lies at or before b's with the one below
+      while(top[s] >= 1 && (Fq - Fb[s]) * (vb[s] - va[s]) <= (Fb[s] - Fa[s]) * (long long)(q - vb[s]))
+      {
+        --top[s];
+        vb[s] = va[s]; Fb[s] = Fa[s];
+        if(top[s] >= 1)
+        {
+          va[s] = stack[s][(size_t)(top[s] - 1) * stride];
+          Fa[s] = (long long)esdf_site(esdf_in<PASS>(P, base + (size_t)va[s] * stride), s) + (long long)va[s] * va[s];
+        }
+      }
+      va[s] = vb[s]; Fa[s] = Fb[s];
+      vb[s] = q; Fb[s] = Fq;
+      ++top[s];
+      stack[s][(size_t)top[s] * stride] = (unsigned short)q;
+    }
+  }
+
+  // phase 2: entry k = (vk, Fk) and k + 1 = (vn, Fn) per set
+  int k[2] = {0, 0}, vk[2] = {0, 0}, vn[2] = {0, 0};
+  long long Fk[2] = {0, 0}, Fn[2] = {0, 0};
+#pragma unroll
+  for(int s = 0; s < 2; ++s)
+    for(int e = 0; e < 2 && e <= top[s]; ++e)
+    {
+      const int v = stack[s][(size_t)e * stride];
+      const long long F = (long long)esdf_site(esdf_in<PASS>(P, base + (size_t)v * stride), s) + (long long)v * v;
+      if(e == 0) { vk[s] = v; Fk[s] = F; }
+      else       { vn[s] = v; Fn[s] = F; }
+    }
+  for(int q = 0; q < n; ++q)
+  {
+    const size_t idx = base + (size_t)q * stride;
+    const int p = esdf_in<PASS>(P, idx);
+    int d = ESDF_INF;
+#pragma unroll
+    for(int s = 0; s < 2; ++s)
+    {
+      if((p < 0) != (s == 1) || top[s] < 0)   // s is not the other set, or it is empty
+        continue;
+      // advance while the intersection of k and k + 1 lies before q: Fn - Fk < 2 q (vn - vk)
+      while(k[s] < top[s] && Fn[s] - Fk[s] < 2ll * q * (vn[s] - vk[s]))
+      {
+        ++k[s];
+        vk[s] = vn[s]; Fk[s] = Fn[s];
+        if(k[s] < top[s])
+        {
+          vn[s] = stack[s][(size_t)(k[s] + 1) * stride];
+          Fn[s] = (long long)esdf_site(esdf_in<PASS>(P, base + (size_t)vn[s] * stride), s) + (long long)vn[s] * vn[s];
+        }
+      }
+      const long long dq = q - vk[s];
+      d = (int)(Fk[s] - (long long)vk[s] * vk[s] + dq * dq);
+    }
+    if(PASS < 2)
+    {
+      P.out[idx] = (int)((p < 0 ? 0x80000000u : 0u) | (unsigned int)d);
+    }
+    else
+    {
+      const float w = __ldg(P.g.vox + idx).y;
+      float dist = d == ESDF_INF ? __int_as_float(0x7f800000) : __fmul_rn(__fsqrt_rn(__int2float_rn(d)), g.voxel);
+      P.esdf[idx] = make_float2(p < 0 ? -dist : dist, w);
+    }
+  }
+}
+
+// One thread per point: the cell of sample_records, then the trilinear distance (x, then y, then z), its analytic
+// gradient in metres and the min corner weight.  Outside the grid: (NaN, 0, 0, 0), weight 0; an infinite corner
+// (O or F empty): its value, gradient 0.
+__global__ void __launch_bounds__(256) volume_esdf_query_kernel(const VolumeEsdfQueryParams Q)
+{
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if(t >= Q.n)
+    return;
+  const float4 p = __ldg(Q.xyzw + t);
+  const float s = Q.voxel;
+  const float gx = __fdiv_rn(__fsub_rn(p.x, Q.ox), s), gy = __fdiv_rn(__fsub_rn(p.y, Q.oy), s),
+              gz = __fdiv_rn(__fsub_rn(p.z, Q.oz), s);
+  const float x0 = floorf(gx), y0 = floorf(gy), z0 = floorf(gz);
+  const int i0 = (x0 >= 0.0f && x0 < 2.0e9f) ? (int)x0 : -1;
+  const int j0 = (y0 >= 0.0f && y0 < 2.0e9f) ? (int)y0 : -1;
+  const int k0 = (z0 >= 0.0f && z0 < 2.0e9f) ? (int)z0 : -1;
+  float4 out = make_float4(__int_as_float(0x7fffffff), 0.0f, 0.0f, 0.0f);
+  float wmin = 0.0f;
+  if(!(i0 < 0 || j0 < 0 || k0 < 0 || i0 + 1 >= Q.nx || j0 + 1 >= Q.ny || k0 + 1 >= Q.nz))
+  {
+    const size_t plane = (size_t)Q.nx * Q.ny, sy = (size_t)Q.nx;
+    const float2 *b = Q.esdf + ((size_t)k0 * Q.ny + j0) * Q.nx + i0;
+    const float2 c000 = __ldg(b), c100 = __ldg(b + 1), c010 = __ldg(b + sy), c110 = __ldg(b + sy + 1);
+    const float2 c001 = __ldg(b + plane), c101 = __ldg(b + plane + 1), c011 = __ldg(b + plane + sy),
+                 c111 = __ldg(b + plane + sy + 1);
+    wmin = fminf(fminf(fminf(fminf(fminf(fminf(fminf(c000.y, c100.y), c010.y), c110.y), c001.y), c101.y), c011.y),
+                 c111.y);
+    const float e[8] = {c000.x, c100.x, c010.x, c110.x, c001.x, c101.x, c011.x, c111.x};
+    bool inf = false;
+#pragma unroll
+    for(int q = 0; q < 8; ++q)
+      if(!inf && (__float_as_uint(e[q]) & 0x7fffffffu) == 0x7f800000u)
+      {
+        out.x = e[q];   // the first infinite corner
+        inf = true;
+      }
+    if(!inf)
+    {
+      const float fx = __fsub_rn(gx, x0), fy = __fsub_rn(gy, y0), fz = __fsub_rn(gz, z0);
+      const float c00 = lerp_rn(c000.x, c100.x, fx), c10 = lerp_rn(c010.x, c110.x, fx);
+      const float c01 = lerp_rn(c001.x, c101.x, fx), c11 = lerp_rn(c011.x, c111.x, fx);
+      out.x = lerp_rn(lerp_rn(c00, c10, fy), lerp_rn(c01, c11, fy), fz);
+      out.y = __fdiv_rn(lerp_rn(lerp_rn(__fsub_rn(c100.x, c000.x), __fsub_rn(c110.x, c010.x), fy),
+                                lerp_rn(__fsub_rn(c101.x, c001.x), __fsub_rn(c111.x, c011.x), fy), fz), s);
+      out.z = __fdiv_rn(lerp_rn(lerp_rn(__fsub_rn(c010.x, c000.x), __fsub_rn(c110.x, c100.x), fx),
+                                lerp_rn(__fsub_rn(c011.x, c001.x), __fsub_rn(c111.x, c101.x), fx), fz), s);
+      out.w = __fdiv_rn(lerp_rn(lerp_rn(__fsub_rn(c001.x, c000.x), __fsub_rn(c101.x, c100.x), fx),
+                                lerp_rn(__fsub_rn(c011.x, c010.x), __fsub_rn(c111.x, c110.x), fx), fy), s);
+    }
+  }
+  Q.dg[t] = out;
+  if(Q.weight)
+    Q.weight[t] = wmin;
+}
+
 } // namespace
 
 cudaError_t launch_volume_integrate(const VolumeIntegrateParams &P, cudaStream_t stream)
@@ -1122,6 +1298,27 @@ cudaError_t launch_volume_store_restore(const VolumeStoreParams &P, unsigned int
     volume_store_restore_kernel<true><<<n, VOLUME_STORE_VOXELS, 0, stream>>>(P);
   else if(n)
     volume_store_restore_kernel<false><<<n, VOLUME_STORE_VOXELS, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_esdf_pass(const VolumeEsdfParams &P, int pass, cudaStream_t stream)
+{
+  const size_t nx = (size_t)P.g.nx, ny = (size_t)P.g.ny, nz = (size_t)P.g.nz;
+  const size_t ncol = pass == 0 ? nx * ny : pass == 1 ? nx * nz : ny * nz;
+  const unsigned int blocks = (unsigned int)((ncol + 255) / 256);
+  if(pass == 0)
+    volume_esdf_kernel<0><<<blocks, 256, 0, stream>>>(P);
+  else if(pass == 1)
+    volume_esdf_kernel<1><<<blocks, 256, 0, stream>>>(P);
+  else
+    volume_esdf_kernel<2><<<blocks, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_esdf_query(const VolumeEsdfQueryParams &Q, cudaStream_t stream)
+{
+  if(Q.n)
+    volume_esdf_query_kernel<<<(unsigned int)((Q.n + 255) / 256), 256, 0, stream>>>(Q);
   return cudaGetLastError();
 }
 

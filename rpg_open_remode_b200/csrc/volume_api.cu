@@ -617,6 +617,25 @@ int store_restore(rmd_volume *v, const int d[3], size_t first, size_t count)
   return 0;
 }
 
+int no_esdf(const char *what)
+{
+  return fail(RMD_ERR_NOT_INITIALISED, (std::string(what) + ": no ESDF has been computed").c_str());
+}
+
+// rmd_volume_esdf_query[_device]: the query kernel on device points / outputs, on the snapshot and its origin.
+int volume_esdf_query(rmd_volume *v, const float4 *xyzw, size_t n, float4 *dg, float *weight)
+{
+  VolumeEsdfQueryParams Q;
+  memset(&Q, 0, sizeof(Q));
+  Q.esdf = v->esdf;
+  Q.nx = v->g.nx; Q.ny = v->g.ny; Q.nz = v->g.nz;
+  Q.voxel = v->g.voxel;
+  Q.ox = v->esdf_o[0]; Q.oy = v->esdf_o[1]; Q.oz = v->esdf_o[2];
+  Q.xyzw = xyzw; Q.dg = dg; Q.weight = weight; Q.n = n;
+  RMD_CUDA_TRY(launch_volume_esdf_query(Q, v->stream));
+  return 0;
+}
+
 // origin + (float)D * s, one rounding per operation as the kernels' voxel_coord (volatile: no contraction)
 float shifted_origin(float origin, long long D, float s)
 {
@@ -688,6 +707,7 @@ int rmd_volume_destroy(rmd_volume_t *v)
     cudaFree(v->store->bricks); cudaFree(v->store->flags);
     delete v->store;
   }
+  cudaFree(v->esdf); cudaFree(v->esdf_scratch);
   cudaGetLastError();
   delete v;
   return 0;
@@ -1185,6 +1205,98 @@ int rmd_volume_upload_store(rmd_volume_t *v, const int64_t *host_coords, const f
   RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
   v->store->index.slot.swap(index.slot);
   return 0;
+}
+
+int rmd_volume_esdf(rmd_volume_t *v)
+{
+  const char *what = "rmd_volume_esdf";
+  VOLUME_REQUIRE(v, "null handle");
+  const long long ex = v->g.nx - 1, ey = v->g.ny - 1, ez = v->g.nz - 1;
+  if(ex * ex + ey * ey + ez * ez >= (1ll << 24))
+    return fail(RMD_ERR_UNSUPPORTED, "rmd_volume_esdf: (nx-1)^2 + (ny-1)^2 + (nz-1)^2 must be < 2^24");
+  DeviceGuard guard(v->device);
+  if(!v->esdf)
+  {
+    float2 *e = NULL;
+    int *s = NULL;
+    cudaError_t err = cudaMalloc(&e, sizeof(float2) * v->n_vox);
+    if(err == cudaSuccess) err = cudaMalloc(&s, 2 * sizeof(int) * v->n_vox);
+    if(err != cudaSuccess)
+    {
+      cudaFree(e); cudaFree(s);
+      cudaGetLastError();
+      return fail_cuda(err, what);
+    }
+    v->esdf = e; v->esdf_scratch = s;
+  }
+  // z: records -> the snapshot's memory (as int32); y: -> the scratch's first half; x: -> the snapshot.  The stacks
+  // are the scratch's second half throughout.
+  VolumeEsdfParams P;
+  memset(&P, 0, sizeof(P));
+  P.g = v->g;
+  P.stack = reinterpret_cast<unsigned short*>(v->esdf_scratch + v->n_vox);
+  P.out = reinterpret_cast<int*>(v->esdf);
+  RMD_CUDA_TRY(launch_volume_esdf_pass(P, 0, v->stream));
+  P.in = P.out;
+  P.out = v->esdf_scratch;
+  RMD_CUDA_TRY(launch_volume_esdf_pass(P, 1, v->stream));
+  P.in = P.out;
+  P.out = NULL;
+  P.esdf = v->esdf;
+  RMD_CUDA_TRY(launch_volume_esdf_pass(P, 2, v->stream));
+  v->esdf_o[0] = v->g.ox; v->esdf_o[1] = v->g.oy; v->esdf_o[2] = v->g.oz;
+  v->esdf_ready = true;
+  return 0;
+}
+
+int rmd_volume_download_esdf(rmd_volume_t *v, float *host_distance, float *host_weight)
+{
+  const char *what = "rmd_volume_download_esdf";
+  VOLUME_REQUIRE(v && host_distance && host_weight, "null argument");
+  if(!v->esdf_ready)
+    return no_esdf(what);
+  DeviceGuard guard(v->device);
+  return volume_download_records(v, v->esdf, host_distance, host_weight, what);
+}
+
+int rmd_volume_esdf_query(rmd_volume_t *v, const float *host_xyzw, size_t n, float *host_dg, float *host_weight)
+{
+  const char *what = "rmd_volume_esdf_query";
+  VOLUME_REQUIRE(v && ((host_xyzw && host_dg) || n == 0), "null argument");
+  VOLUME_REQUIRE(n < ((size_t)1 << 39), "too many points");
+  if(!v->esdf_ready)
+    return no_esdf(what);
+  if(!n)
+    return 0;
+  DeviceGuard guard(v->device);
+  // staging: the points, then the (distance, gradient) and the weights
+  const size_t pts = sizeof(float4) * n, wts = host_weight ? sizeof(float) * n : 0;
+  int rc = volume_grow(&v->stage, &v->stage_cap, 2 * pts + wts);
+  if(rc) return rc;
+  float4 *d_xyzw = reinterpret_cast<float4*>(v->stage), *d_dg = d_xyzw + n;
+  float *d_w = host_weight ? reinterpret_cast<float*>(d_dg + n) : NULL;
+  RMD_CUDA_TRY(cudaMemcpyAsync(d_xyzw, host_xyzw, pts, cudaMemcpyHostToDevice, v->stream));
+  rc = volume_esdf_query(v, d_xyzw, n, d_dg, d_w);
+  if(rc) return rc;
+  RMD_CUDA_TRY(cudaMemcpyAsync(host_dg, d_dg, pts, cudaMemcpyDeviceToHost, v->stream));
+  if(host_weight)
+    RMD_CUDA_TRY(cudaMemcpyAsync(host_weight, d_w, wts, cudaMemcpyDeviceToHost, v->stream));
+  RMD_CUDA_TRY(cudaStreamSynchronize(v->stream));
+  return 0;
+}
+
+int rmd_volume_esdf_query_device(rmd_volume_t *v, const float *dev_xyzw, size_t n, float *dev_dg, float *dev_weight)
+{
+  const char *what = "rmd_volume_esdf_query_device";
+  VOLUME_REQUIRE(v && ((dev_xyzw && dev_dg) || n == 0), "null argument");
+  VOLUME_REQUIRE(n < ((size_t)1 << 39), "too many points");
+  VOLUME_REQUIRE(((uintptr_t)dev_xyzw % 16) == 0 && ((uintptr_t)dev_dg % 16) == 0 && ((uintptr_t)dev_weight % 4) == 0,
+                 "points and outputs must be 16-byte (weights 4-byte) aligned");
+  if(!v->esdf_ready)
+    return no_esdf(what);
+  DeviceGuard guard(v->device);
+  return volume_esdf_query(v, reinterpret_cast<const float4*>(dev_xyzw), n, reinterpret_cast<float4*>(dev_dg),
+                           dev_weight);
 }
 
 } // extern "C"

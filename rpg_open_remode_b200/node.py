@@ -31,11 +31,13 @@ class DepthmapNode:
     def __init__(self, depthmap: Depthmap, ref_compl_perc: float = 10.0, max_dist_from_ref: float = 0.5,
                  publish_conv_every_n: int = 10, publisher: Optional[Callable] = None,
                  volume: Optional[TsdfVolume] = None, prior_from_volume: float = 0.0, follow_volume: bool = False,
-                 scene_mesh: Optional[SceneMesh] = None):
+                 scene_mesh: Optional[SceneMesh] = None, esdf: bool = False):
         if prior_from_volume and volume is None:
             raise ValueError("DepthmapNode: prior_from_volume needs a volume")
         if follow_volume and volume is None:
             raise ValueError("DepthmapNode: follow_volume needs a volume")
+        if esdf and volume is None:
+            raise ValueError("DepthmapNode: esdf needs a volume")
         if scene_mesh is not None and not follow_volume:
             raise ValueError("DepthmapNode: scene_mesh needs follow_volume=True")
         if scene_mesh is not None and getattr(volume, "store", False):
@@ -53,6 +55,9 @@ class DepthmapNode:
         # when given, the spill mesh of every shift is added to it, so that scene_mesh.mesh(volume) meshes the whole
         # traversed scene
         self.scene_mesh_ = scene_mesh
+        # when set, the volume's ESDF is recomputed after each keyframe is fused and published as ("volume_esdf",
+        # volume), ready for esdfQuery
+        self.esdf_ = bool(esdf)
         self.ref_depth_range_ = (0.0, 0.0)   # [min_depth, max_depth] of the current keyframe
         self.state_ = TAKE_REFERENCE_FRAME                      # src/depthmap_node.cpp:35
         self.ref_compl_perc_ = float(ref_compl_perc)            # :81, default 10.0
@@ -94,6 +99,10 @@ class DepthmapNode:
         self.depthmap_.downloadConvergenceMap()                                   # :168
         if self.publisher_:
             self.publisher_("depthmap_and_pointcloud", self.depthmap_)
+        if self.esdf_:
+            self.volume_.computeEsdf()
+            if self.publisher_:
+                self.publisher_("volume_esdf", self.volume_)
 
     def followVolume(self) -> None:
         """Recentre volume_ on the finished keyframe's view centre -- the camera centre plus the middle of
