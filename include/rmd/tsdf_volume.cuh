@@ -254,7 +254,19 @@ public:
   // when one set is empty.  Asynchronous; the snapshot and its origin stay until the next computeEsdf().  The first
   // call allocates 16 B per voxel.  Throws past (nx-1)^2 + (ny-1)^2 + (nz-1)^2 >= 2^24.
   void computeEsdf() { detail::throw_on_error(rmd_volume_esdf(handle_), "TsdfVolume: unable to compute the ESDF"); }
-  // The snapshot's distance and weight, nx * ny * nz floats each.
+  // The same over a box of the map: lower corner lo (window indices, may lie outside the window) and dims; each box
+  // voxel takes the window's record, else its stored brick's, else unknown (rmd_volume_esdf_box).  24 B per box voxel.
+  void computeEsdf(const int64_t lo[3], const int dims[3])
+  {
+    detail::throw_on_error(rmd_volume_esdf_box(handle_, lo, dims), "TsdfVolume: unable to compute the ESDF of a box");
+  }
+  // The box the snapshot answers for: lowest unbounded voxel, dims and origin (any may be NULL).
+  void esdfInfo(int64_t lo_unbounded[3], int dims[3], float origin[3])
+  {
+    detail::throw_on_error(rmd_volume_esdf_info(handle_, lo_unbounded, dims, origin),
+                           "TsdfVolume: unable to read the ESDF's box");
+  }
+  // The snapshot's distance and weight, one float each per voxel of its box (nx * ny * nz for the window's).
   void downloadEsdf(float *host_distance, float *host_weight)
   {
     detail::throw_on_error(rmd_volume_download_esdf(handle_, host_distance, host_weight),

@@ -771,11 +771,11 @@ int rmd_volume_upload_store(rmd_volume_t *v, const int64_t *host_coords, const f
  * -inf when F is empty; weight = the record's weight, bit for bit, at the
  * time of the call (0 = unknown).  Obstacles in the brick store or outside the
  * window are not seen, so near the window's faces a distance is an upper
- * bound.  Requires (nx-1)^2 + (ny-1)^2 + (nz-1)^2 < 2^24 (every squared
+ * bound (rmd_volume_esdf_box, below, computes a box of the map instead).  Requires (nx-1)^2 + (ny-1)^2 + (nz-1)^2 < 2^24 (every squared
  * distance exact in fp32): RMD_ERR_UNSUPPORTED otherwise.
  *   Memory: 16 B per voxel -- the 8 B snapshot and 8 B of scratch --
- * allocated by the first compute (cudaErrorMemoryAllocation when it does not
- * fit) and freed by rmd_volume_destroy; 2 GiB at 512^3.  A volume that never
+ * allocated by the first compute that needs them (cudaErrorMemoryAllocation
+ * when it does not fit) and freed by rmd_volume_destroy; 2 GiB at 512^3.  A volume that never
  * computes an ESDF allocates nothing.
  *   Only a compute writes the snapshot: later integrations, shifts, uploads
  * and resets leave it and its origin as they were, so queries answer for the
@@ -799,8 +799,41 @@ int rmd_volume_upload_store(rmd_volume_t *v, const int64_t *host_coords, const f
  * RMD_ERR_INVALID_ARGUMENT: null handle or pointer (n = 0 allows NULL
  * points and outputs), misaligned device pointers. */
 int rmd_volume_esdf(rmd_volume_t *v);
+/* The ESDF of a box of the map that the caller chooses (DESIGN.md 4.8), so
+ * that obstacles in the brick store and points outside the window count.
+ *   Box: lower corner lo (int64, window indices at the time of the call; it
+ * may be negative and may lie outside the window) and dims m (each > 0).  Box
+ * voxel (i, j, k) is voxel D + lo + (i, j, k) of the unbounded grid, D the
+ * total offset (rmd_volume_offset).  Its record is the window's when the
+ * voxel lies in the window; otherwise, on a volume with the store, the stored
+ * brick's when its brick floor(u / 8) is stored (stale copies of bricks back
+ * in the window are never read); otherwise (0, 0), unknown.
+ *   The snapshot is rmd_volume_esdf's definition applied to those records
+ * with dims m: the same sets, +inf / -inf rules, fp32 expressions, and the
+ * weight copied bit for bit.  Its origin is o0 + (float)(D + lo) * s per axis
+ * (o0 the creation origin; rmd_volume_shift's rounding), and for lo = 0 the
+ * window's origin itself, so the box (0, n) gives rmd_volume_esdf's snapshot,
+ * origin and queries bit for bit.  Obstacles outside the box are not seen, so
+ * near its faces a distance is an upper bound.  Queries and downloads then
+ * answer for the box.
+ *   Memory: 24 B per box voxel -- rmd_volume_esdf's 16 B and 8 B of gathered
+ * records -- plus, with the store, 4 B per brick of the box for the brick
+ * table, all grown on demand: new buffers are allocated before old ones are
+ * freed, so cudaErrorMemoryAllocation leaves the previous snapshot intact and
+ * queryable.  The snapshot semantics and stream ordering are rmd_volume_esdf's
+ * (asynchronous, no host synchronisation).
+ *   RMD_ERR_UNSUPPORTED: (mx-1)^2 + (my-1)^2 + (mz-1)^2 >= 2^24.
+ * RMD_ERR_INVALID_ARGUMENT: null handle or pointer, a dimension <= 0, or
+ * D + lo + m overflowing int64. */
+int rmd_volume_esdf_box(rmd_volume_t *v, const int64_t lo[3], const int dims[3]);
+/* The box the snapshot answers for: its lowest unbounded voxel D + lo (D at
+ * the compute), its dims and its origin (the window's for rmd_volume_esdf).
+ * Any output may be NULL.  RMD_ERR_NOT_INITIALISED before the first
+ * compute. */
+int rmd_volume_esdf_info(rmd_volume_t *v, int64_t lo_unbounded[3], int dims[3], float origin[3]);
 /* Test / checkpoint hook (like rmd_volume_download): the snapshot's distance
- * and weight, nx * ny * nz floats each.  Synchronous. */
+ * and weight, one float each per voxel of the snapshot (mx * my * mz, the
+ * window's nx * ny * nz for rmd_volume_esdf), x fastest.  Synchronous. */
 int rmd_volume_download_esdf(rmd_volume_t *v, float *host_distance, float *host_weight);
 int rmd_volume_esdf_query(rmd_volume_t *v, const float *host_xyzw, size_t n, float *host_dg, float *host_weight);
 int rmd_volume_esdf_query_device(rmd_volume_t *v, const float *dev_xyzw, size_t n, float *dev_dg, float *dev_weight);

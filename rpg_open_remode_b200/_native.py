@@ -111,6 +111,8 @@ _SIGNATURES = {
     "rmd_volume_download_store": (ci, [vp, vp, vp, vp, vp, vp, cs, P(cs)]),
     "rmd_volume_upload_store": (ci, [vp, vp, vp, vp, vp, vp, cs]),
     "rmd_volume_esdf": (ci, [vp]),
+    "rmd_volume_esdf_box": (ci, [vp, vp, vp]),
+    "rmd_volume_esdf_info": (ci, [vp, vp, vp, vp]),
     "rmd_volume_download_esdf": (ci, [vp, vp, vp]),
     "rmd_volume_esdf_query": (ci, [vp, vp, cs, vp, vp]),
     "rmd_volume_esdf_query_device": (ci, [vp, vp, cs, vp, vp]),

@@ -870,19 +870,50 @@ class TsdfVolume:
         return (np.concatenate(V)[keep], tri.reshape(-1, 3),
                 np.concatenate(I)[keep] if intensity else None, np.concatenate(N)[keep] if normals else None)
 
-    def computeEsdf(self) -> None:
+    def computeEsdf(self, lo=None, dims=None) -> None:
         """Compute the Euclidean signed distance field of the current window (DESIGN.md 4.8): per voxel the distance
         in metres to the nearest occupied voxel (weight > 0 and tsdf <= 0) for a free or unknown voxel, minus the
         distance to the nearest other voxel for an occupied one; +inf / -inf everywhere when no voxel is occupied /
         free.  Obstacles outside the window are not seen.  Asynchronous on the volume's stream; the snapshot and its
         origin stay as they are until the next computeEsdf(), whatever the volume does meanwhile.  The first call
-        allocates 16 B per voxel.  Raises RmdError (RMD_ERR_UNSUPPORTED) unless (nx-1)^2 + (ny-1)^2 + (nz-1)^2 < 2^24."""
-        check(self._L.rmd_volume_esdf(self._h), "TsdfVolume::computeEsdf")
+        allocates 16 B per voxel.  Raises RmdError (RMD_ERR_UNSUPPORTED) unless (nx-1)^2 + (ny-1)^2 + (nz-1)^2 < 2^24.
+
+        With lo (int [3], window indices, may be negative or outside the window) and dims (int [3], each > 0): the
+        same over that box of the map.  Each box voxel takes the window's record, else (with the store) its stored
+        brick's, else unknown; the snapshot's origin is origin + lo * voxel_size from the creation origin and the
+        total offset, so esdfQuery answers around the box and obstacles in the store count.  24 B per box voxel.
+        esdfBox() tells which box the snapshot answers for."""
+        if lo is None and dims is None:
+            check(self._L.rmd_volume_esdf(self._h), "TsdfVolume::computeEsdf")
+            return
+        what = "TsdfVolume::computeEsdf"
+        if lo is None or dims is None:
+            raise ValueError(what + ": lo and dims come together")
+        a, m = list(np.asarray(lo).reshape(-1)), list(np.asarray(dims).reshape(-1))
+        if len(a) != 3 or len(m) != 3 or any(int(x) != x for x in a + m):
+            raise ValueError(what + ": lo and dims must be three whole numbers each")
+        if any(not -2 ** 63 <= int(x) < 2 ** 63 for x in a) or any(not -2 ** 31 <= int(x) < 2 ** 31 for x in m):
+            raise ValueError(what + ": lo must fit int64 and dims int32")
+        lo64 = np.array([int(x) for x in a], np.int64)
+        m32 = np.array([int(x) for x in m], np.int32)
+        check(self._L.rmd_volume_esdf_box(self._h, lo64.ctypes.data, m32.ctypes.data), what)
+
+    def esdfBox(self):
+        """(lo_unbounded int64 [3], dims (mx, my, mz), origin float32 [3]) of the box the snapshot answers for: its
+        lowest voxel of the unbounded grid (offset + lo at the compute), its size and the world position of its voxel
+        (0, 0, 0).  The window's box after computeEsdf()."""
+        lo, m, o = np.empty(3, np.int64), np.empty(3, np.int32), np.empty(3, np.float32)
+        check(self._L.rmd_volume_esdf_info(self._h, lo.ctypes.data, m.ctypes.data, o.ctypes.data),
+              "TsdfVolume::esdfBox")
+        return lo, tuple(int(x) for x in m), o
 
     def downloadEsdf(self):
-        """(distance, weight) of the snapshot, float32 arrays of shape (nz, ny, nx); weight = the records' weight at
-        the compute (0 = unknown)."""
-        return self._download_records(self._L.rmd_volume_download_esdf, "TsdfVolume::downloadEsdf")
+        """(distance, weight) of the snapshot, float32 arrays of shape (mz, my, mx), the dims of its box (the
+        window's after computeEsdf()); weight = the records' weight at the compute (0 = unknown)."""
+        _, (mx, my, mz), _ = self.esdfBox()
+        a, b = np.empty((mz, my, mx), np.float32), np.empty((mz, my, mx), np.float32)
+        check(self._L.rmd_volume_download_esdf(self._h, a.ctypes.data, b.ctypes.data), "TsdfVolume::downloadEsdf")
+        return a, b
 
     def esdfQuery(self, points):
         """(dg float32 [N, 4] = (distance, d/dx, d/dy, d/dz), weight float32 [N]) at world points [N, 3] or [N, 4]

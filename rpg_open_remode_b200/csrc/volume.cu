@@ -1134,6 +1134,26 @@ __global__ void __launch_bounds__(256) volume_esdf_query_kernel(const VolumeEsdf
     Q.weight[t] = wmin;
 }
 
+// One thread per box voxel: blockIdx.y / z = j / k, x fastest.  A window voxel is one __ldg of its record; any other
+// looks up its brick in the table and, when stored, loads the brick's record (store_moving_voxel's layout).
+__global__ void __launch_bounds__(128) volume_esdf_gather_kernel(const VolumeEsdfGatherParams P)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y, k = blockIdx.z;
+  if(i >= P.mx)
+    return;
+  float2 r = make_float2(0.0f, 0.0f);
+  if(i >= P.wlo[0] && i < P.whi[0] && j >= P.wlo[1] && j < P.whi[1] && k >= P.wlo[2] && k < P.whi[2])
+    r = __ldg(P.g.vox + ((size_t)(k + P.wof[2]) * P.g.ny + (j + P.wof[1])) * P.g.nx + (i + P.wof[0]));
+  else if(P.table)
+  {
+    const int ux = P.r[0] + i, uy = P.r[1] + j, uz = P.r[2] + k;
+    const int slot = __ldg(P.table + ((size_t)(uz >> 3) * P.tb[1] + (uy >> 3)) * P.tb[0] + (ux >> 3));
+    if(slot >= 0)
+      r = __ldg(P.pool + (size_t)slot * VOLUME_STORE_VOXELS + ((ux & 7) + 8 * (uy & 7) + 64 * (uz & 7)));
+  }
+  P.out[((size_t)k * P.my + j) * P.mx + i] = r;
+}
+
 } // namespace
 
 cudaError_t launch_volume_integrate(const VolumeIntegrateParams &P, cudaStream_t stream)
@@ -1312,6 +1332,13 @@ cudaError_t launch_volume_esdf_pass(const VolumeEsdfParams &P, int pass, cudaStr
     volume_esdf_kernel<1><<<blocks, 256, 0, stream>>>(P);
   else
     volume_esdf_kernel<2><<<blocks, 256, 0, stream>>>(P);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_volume_esdf_gather(const VolumeEsdfGatherParams &P, cudaStream_t stream)
+{
+  const dim3 grid((unsigned int)((P.mx + 127) / 128), (unsigned int)P.my, (unsigned int)P.mz);
+  volume_esdf_gather_kernel<<<grid, 128, 0, stream>>>(P);
   return cudaGetLastError();
 }
 

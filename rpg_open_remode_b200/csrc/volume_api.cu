@@ -321,16 +321,17 @@ int volume_raycast_normals(const char *what, rmd_volume_t *v, int width, int hei
   return 0;
 }
 
-// A record array (g.vox or col) to two host arrays of n_vox floats (.x to a, .y to b), through host chunks.
-int volume_download_records(rmd_volume *v, const float2 *records, float *a, float *b, const char *what)
+// A record array of n float2 (g.vox, col or the ESDF snapshot) to two host arrays of n floats (.x to a, .y to b),
+// through host chunks.
+int volume_download_records(rmd_volume *v, const float2 *records, size_t n, float *a, float *b, const char *what)
 {
-  const size_t chunk = v->n_vox < kVolumeChunk ? v->n_vox : kVolumeChunk;
+  const size_t chunk = n < kVolumeChunk ? n : kVolumeChunk;
   float2 *tmp = static_cast<float2*>(malloc(sizeof(float2) * chunk));
   if(!tmp) return fail((int)cudaErrorMemoryAllocation, (std::string(what) + ": host allocation failed").c_str());
   cudaError_t err = cudaSuccess;
-  for(size_t c = 0; c < v->n_vox && err == cudaSuccess; c += chunk)
+  for(size_t c = 0; c < n && err == cudaSuccess; c += chunk)
   {
-    const size_t m = v->n_vox - c < chunk ? v->n_vox - c : chunk;
+    const size_t m = n - c < chunk ? n - c : chunk;
     err = cudaMemcpyAsync(tmp, records + c, sizeof(float2) * m, cudaMemcpyDeviceToHost, v->stream);
     if(err == cudaSuccess) err = cudaStreamSynchronize(v->stream);
     for(size_t q = 0; q < m && err == cudaSuccess; ++q)
@@ -628,7 +629,7 @@ int volume_esdf_query(rmd_volume *v, const float4 *xyzw, size_t n, float4 *dg, f
   VolumeEsdfQueryParams Q;
   memset(&Q, 0, sizeof(Q));
   Q.esdf = v->esdf;
-  Q.nx = v->g.nx; Q.ny = v->g.ny; Q.nz = v->g.nz;
+  Q.nx = v->esdf_dims[0]; Q.ny = v->esdf_dims[1]; Q.nz = v->esdf_dims[2];
   Q.voxel = v->g.voxel;
   Q.ox = v->esdf_o[0]; Q.oy = v->esdf_o[1]; Q.oz = v->esdf_o[2];
   Q.xyzw = xyzw; Q.dg = dg; Q.weight = weight; Q.n = n;
@@ -641,6 +642,74 @@ float shifted_origin(float origin, long long D, float s)
 {
   volatile float step = (float)D * s;
   return origin + step;
+}
+
+// The ESDF buffers for a snapshot of n voxels, with the gathered records of a box (records) and a brick table of
+// `table` entries (0: none).  Every new buffer is allocated before any old one is freed, so that a failure leaves the
+// previous snapshot as it was; a snapshot whose buffer is replaced is gone until the compute that follows.
+int esdf_reserve(rmd_volume *v, size_t n, bool records, size_t table, const char *what)
+{
+  const bool grow = n > v->esdf_cap, grow_rec = records && n > v->esdf_rec_cap, grow_table = table > v->esdf_table_cap;
+  float2 *e = NULL, *r = NULL;
+  int *s = NULL, *t = NULL;
+  cudaError_t err = cudaSuccess;
+  if(grow) err = cudaMalloc(&e, sizeof(float2) * n);
+  if(err == cudaSuccess && grow) err = cudaMalloc(&s, 2 * sizeof(int) * n);
+  if(err == cudaSuccess && grow_rec) err = cudaMalloc(&r, sizeof(float2) * n);
+  if(err == cudaSuccess && grow_table) err = cudaMalloc(&t, sizeof(int) * table);
+  if(err != cudaSuccess)
+  {
+    cudaFree(e); cudaFree(s); cudaFree(r); cudaFree(t);
+    cudaGetLastError();
+    return fail_cuda(err, what);
+  }
+  if(grow)
+  {
+    cudaFree(v->esdf); cudaFree(v->esdf_scratch);
+    v->esdf = e; v->esdf_scratch = s; v->esdf_cap = n;
+    v->esdf_ready = false;
+  }
+  if(grow_rec)
+  {
+    cudaFree(v->esdf_rec);
+    v->esdf_rec = r; v->esdf_rec_cap = n;
+  }
+  if(grow_table)
+  {
+    cudaFree(v->esdf_table);
+    v->esdf_table = t; v->esdf_table_cap = table;
+  }
+  return 0;
+}
+
+// The three passes on the records of g (the window's or a box's) into the snapshot, which then answers for g's dims,
+// the unbounded lower corner lo and origin o.
+int esdf_passes(rmd_volume *v, const VolumeGrid &g, const long long lo[3], const float o[3])
+{
+  const size_t n = (size_t)g.nx * (size_t)g.ny * (size_t)g.nz;
+  // z: records -> the snapshot's memory (as int32); y: -> the scratch's first half; x: -> the snapshot.  The stacks
+  // are the scratch from n on throughout.
+  VolumeEsdfParams P;
+  memset(&P, 0, sizeof(P));
+  P.g = g;
+  P.stack = reinterpret_cast<unsigned short*>(v->esdf_scratch + n);
+  P.out = reinterpret_cast<int*>(v->esdf);
+  RMD_CUDA_TRY(launch_volume_esdf_pass(P, 0, v->stream));
+  P.in = P.out;
+  P.out = v->esdf_scratch;
+  RMD_CUDA_TRY(launch_volume_esdf_pass(P, 1, v->stream));
+  P.in = P.out;
+  P.out = NULL;
+  P.esdf = v->esdf;
+  RMD_CUDA_TRY(launch_volume_esdf_pass(P, 2, v->stream));
+  v->esdf_dims[0] = g.nx; v->esdf_dims[1] = g.ny; v->esdf_dims[2] = g.nz;
+  for(int a = 0; a < 3; ++a)
+  {
+    v->esdf_lo[a] = lo[a];
+    v->esdf_o[a] = o[a];
+  }
+  v->esdf_ready = true;
+  return 0;
 }
 
 } // namespace
@@ -707,7 +776,7 @@ int rmd_volume_destroy(rmd_volume_t *v)
     cudaFree(v->store->bricks); cudaFree(v->store->flags);
     delete v->store;
   }
-  cudaFree(v->esdf); cudaFree(v->esdf_scratch);
+  cudaFree(v->esdf); cudaFree(v->esdf_scratch); cudaFree(v->esdf_rec); cudaFree(v->esdf_table);
   cudaGetLastError();
   delete v;
   return 0;
@@ -1051,7 +1120,7 @@ int rmd_volume_download(rmd_volume_t *v, float *host_tsdf, float *host_weight)
 {
   RMD_REQUIRE(v && host_tsdf && host_weight, "rmd_volume_download: null argument");
   DeviceGuard guard(v->device);
-  return volume_download_records(v, v->g.vox, host_tsdf, host_weight, "rmd_volume_download");
+  return volume_download_records(v, v->g.vox, v->n_vox, host_tsdf, host_weight, "rmd_volume_download");
 }
 
 int rmd_volume_upload(rmd_volume_t *v, const float *host_tsdf, const float *host_weight)
@@ -1067,7 +1136,7 @@ int rmd_volume_download_intensity(rmd_volume_t *v, float *host_intensity, float 
   if(!v->col)
     return no_intensity("rmd_volume_download_intensity");
   DeviceGuard guard(v->device);
-  return volume_download_records(v, v->col, host_intensity, host_weight, "rmd_volume_download_intensity");
+  return volume_download_records(v, v->col, v->n_vox, host_intensity, host_weight, "rmd_volume_download_intensity");
 }
 
 int rmd_volume_upload_intensity(rmd_volume_t *v, const float *host_intensity, const float *host_weight)
@@ -1215,37 +1284,98 @@ int rmd_volume_esdf(rmd_volume_t *v)
   if(ex * ex + ey * ey + ez * ez >= (1ll << 24))
     return fail(RMD_ERR_UNSUPPORTED, "rmd_volume_esdf: (nx-1)^2 + (ny-1)^2 + (nz-1)^2 must be < 2^24");
   DeviceGuard guard(v->device);
-  if(!v->esdf)
+  // the window's records as they are: no gather
+  const int rc = esdf_reserve(v, v->n_vox, false, 0, what);
+  if(rc) return rc;
+  const float o[3] = {v->g.ox, v->g.oy, v->g.oz};
+  return esdf_passes(v, v->g, v->D, o);
+}
+
+int rmd_volume_esdf_box(rmd_volume_t *v, const int64_t lo[3], const int dims[3])
+{
+  const char *what = "rmd_volume_esdf_box";
+  VOLUME_REQUIRE(v && lo && dims, "null argument");
+  VOLUME_REQUIRE(dims[0] > 0 && dims[1] > 0 && dims[2] > 0, "box dimensions must be positive");
+  const int n[3] = {v->g.nx, v->g.ny, v->g.nz};
+  long long base[3], end[3];   // the box's unbounded voxels [D + lo, D + lo + dims)
+  for(int a = 0; a < 3; ++a)
+    VOLUME_REQUIRE(!__builtin_add_overflow(v->D[a], (long long)lo[a], &base[a]) &&
+                   !__builtin_add_overflow(base[a], (long long)dims[a], &end[a]),
+                   "the total offset plus the box's corner and size overflows");
+  const long long ex = dims[0] - 1, ey = dims[1] - 1, ez = dims[2] - 1;
+  if(ex * ex + ey * ey + ez * ez >= (1ll << 24))
+    return fail(RMD_ERR_UNSUPPORTED, "rmd_volume_esdf_box: (mx-1)^2 + (my-1)^2 + (mz-1)^2 must be < 2^24");
+  VolumeEsdfGatherParams G;
+  memset(&G, 0, sizeof(G));
+  G.g = v->g;
+  G.mx = dims[0]; G.my = dims[1]; G.mz = dims[2];
+  // the window's part, box index i = window index - lo: [max(0, -lo), min(m, n - lo)) when lo lies in (-m, n)
+  bool meets = true, inside = true;
+  for(int a = 0; a < 3; ++a)
+    meets = meets && lo[a] < n[a] && lo[a] > -(long long)dims[a];
+  for(int a = 0; meets && a < 3; ++a)
   {
-    float2 *e = NULL;
-    int *s = NULL;
-    cudaError_t err = cudaMalloc(&e, sizeof(float2) * v->n_vox);
-    if(err == cudaSuccess) err = cudaMalloc(&s, 2 * sizeof(int) * v->n_vox);
-    if(err != cudaSuccess)
-    {
-      cudaFree(e); cudaFree(s);
-      cudaGetLastError();
-      return fail_cuda(err, what);
-    }
-    v->esdf = e; v->esdf_scratch = s;
+    const int l = (int)lo[a];
+    const long long h = (long long)n[a] - l;
+    G.wlo[a] = l < 0 ? -l : 0;
+    G.whi[a] = h < dims[a] ? (int)h : dims[a];
+    G.wof[a] = l;
+    inside = inside && G.wlo[a] == 0 && G.whi[a] == dims[a];
   }
-  // z: records -> the snapshot's memory (as int32); y: -> the scratch's first half; x: -> the snapshot.  The stacks
-  // are the scratch's second half throughout.
-  VolumeEsdfParams P;
-  memset(&P, 0, sizeof(P));
-  P.g = v->g;
-  P.stack = reinterpret_cast<unsigned short*>(v->esdf_scratch + v->n_vox);
-  P.out = reinterpret_cast<int*>(v->esdf);
-  RMD_CUDA_TRY(launch_volume_esdf_pass(P, 0, v->stream));
-  P.in = P.out;
-  P.out = v->esdf_scratch;
-  RMD_CUDA_TRY(launch_volume_esdf_pass(P, 1, v->stream));
-  P.in = P.out;
-  P.out = NULL;
-  P.esdf = v->esdf;
-  RMD_CUDA_TRY(launch_volume_esdf_pass(P, 2, v->stream));
-  v->esdf_o[0] = v->g.ox; v->esdf_o[1] = v->g.oy; v->esdf_o[2] = v->g.oz;
-  v->esdf_ready = true;
+  inside = meets && inside;
+  // the brick table over the box's bricks [floor(base / 8), floor((end - 1) / 8)]
+  std::vector<int> table;
+  const bool lookup = v->store && !v->store->index.slot.empty() && !inside;
+  if(lookup)
+  {
+    int64_t b0[3];
+    int nb[3];
+    for(int a = 0; a < 3; ++a)
+    {
+      b0[a] = brick_floor(base[a]);
+      nb[a] = (int)(brick_floor(end[a] - 1) - b0[a] + 1);
+      G.r[a] = (int)(base[a] - b0[a] * STORE_BRICK);
+      G.tb[a] = nb[a];
+    }
+    table = store_brick_table(v->store->index, b0, nb);
+  }
+  DeviceGuard guard(v->device);
+  const size_t m = (size_t)dims[0] * (size_t)dims[1] * (size_t)dims[2];
+  int rc = esdf_reserve(v, m, true, table.size(), what);
+  if(rc) return rc;
+  if(lookup)
+  {
+    // pageable source: the copy is staged before the call returns
+    RMD_CUDA_TRY(cudaMemcpyAsync(v->esdf_table, table.data(), sizeof(int) * table.size(), cudaMemcpyHostToDevice,
+                                 v->stream));
+    G.table = v->esdf_table;
+    G.pool = v->store->pool;
+  }
+  G.out = v->esdf_rec;
+  RMD_CUDA_TRY(launch_volume_esdf_gather(G, v->stream));
+  VolumeGrid B = v->g;
+  B.vox = v->esdf_rec;
+  B.nx = dims[0]; B.ny = dims[1]; B.nz = dims[2];
+  const float og[3] = {v->g.ox, v->g.oy, v->g.oz};
+  float o[3];
+  for(int a = 0; a < 3; ++a)   // lo = 0: the window's origin itself
+    o[a] = lo[a] == 0 ? og[a] : shifted_origin(v->o0[a], base[a], v->g.voxel);
+  B.ox = o[0]; B.oy = o[1]; B.oz = o[2];
+  return esdf_passes(v, B, base, o);
+}
+
+int rmd_volume_esdf_info(rmd_volume_t *v, int64_t lo_unbounded[3], int dims[3], float origin[3])
+{
+  const char *what = "rmd_volume_esdf_info";
+  VOLUME_REQUIRE(v, "null handle");
+  if(!v->esdf_ready)
+    return no_esdf(what);
+  for(int a = 0; a < 3; ++a)
+  {
+    if(lo_unbounded) lo_unbounded[a] = v->esdf_lo[a];
+    if(dims) dims[a] = v->esdf_dims[a];
+    if(origin) origin[a] = v->esdf_o[a];
+  }
   return 0;
 }
 
@@ -1256,7 +1386,8 @@ int rmd_volume_download_esdf(rmd_volume_t *v, float *host_distance, float *host_
   if(!v->esdf_ready)
     return no_esdf(what);
   DeviceGuard guard(v->device);
-  return volume_download_records(v, v->esdf, host_distance, host_weight, what);
+  const size_t n = (size_t)v->esdf_dims[0] * (size_t)v->esdf_dims[1] * (size_t)v->esdf_dims[2];
+  return volume_download_records(v, v->esdf, n, host_distance, host_weight, what);
 }
 
 int rmd_volume_esdf_query(rmd_volume_t *v, const float *host_xyzw, size_t n, float *host_dg, float *host_weight)

@@ -103,6 +103,28 @@ struct BrickIndex
   }
 };
 
+// The brick table of an ESDF box (DESIGN.md 4.8): nb[0] * nb[1] * nb[2] entries, x fastest, for the bricks
+// [b0, b0 + nb) per axis of the unbounded grid; each stored brick in that range holds its pool slot, every other entry
+// -1.
+inline std::vector<int> store_brick_table(const BrickIndex &index, const int64_t b0[3], const int nb[3])
+{
+  std::vector<int> table((size_t)nb[0] * (size_t)nb[1] * (size_t)nb[2], -1);
+  for(const auto &e : index.slot)
+  {
+    uint64_t t[3];
+    bool inside = true;
+    for(int a = 0; a < 3; ++a)
+    {
+      // b >= b0 makes the unsigned difference exact
+      t[a] = (uint64_t)e.first.b[a] - (uint64_t)b0[a];
+      inside = inside && e.first.b[a] >= b0[a] && t[a] < (uint64_t)nb[a];
+    }
+    if(inside)
+      table[(t[2] * (uint64_t)nb[1] + t[1]) * (uint64_t)nb[0] + t[0]] = e.second;
+  }
+  return table;
+}
+
 // Pool capacity (bricks) for `need` bricks from `cap`: doubled until it fits, at least 64.
 inline size_t store_pool_capacity(size_t cap, size_t need)
 {

@@ -22,6 +22,17 @@ from .api import PRIOR_SIGMA_SQ_FRAC, SE3, Depthmap, SceneMesh, SeedMatrix, Tsdf
 UPDATE, TAKE_REFERENCE_FRAME = 0, 1   # rmd::ProcessingStates::State, include/rmd/depthmap_node.h:32-36
 
 
+def esdf_camera_box(dims, voxel_size: float, origin, camera_centre, margin: int):
+    """DepthmapNode's ESDF box with esdf_camera_margin = margin > 0: (lo int64 [3], dims int64 [3]) in window indices,
+    the bounding box of the window [0, dims) and of [c - margin, c + margin] with c = round((camera_centre - origin) /
+    voxel_size) in float64, followVolume's conversion to window indices."""
+    c = np.round((np.asarray(camera_centre, np.float64) - np.asarray(origin, np.float32).astype(np.float64))
+                 / float(voxel_size)).astype(np.int64)
+    n = np.asarray(dims, np.int64)
+    lo = np.minimum(0, c - int(margin))
+    return lo, np.maximum(n, c + int(margin) + 1) - lo
+
+
 class DepthmapNode:
     """rmd::DepthmapNode::denseInputCallback with the ROS plumbing removed.  `publisher` receives
     ("depthmap_and_pointcloud", depthmap) after a keyframe is finished (denoiseAndPublishResults,
@@ -31,7 +42,11 @@ class DepthmapNode:
     def __init__(self, depthmap: Depthmap, ref_compl_perc: float = 10.0, max_dist_from_ref: float = 0.5,
                  publish_conv_every_n: int = 10, publisher: Optional[Callable] = None,
                  volume: Optional[TsdfVolume] = None, prior_from_volume: float = 0.0, follow_volume: bool = False,
-                 scene_mesh: Optional[SceneMesh] = None, esdf: bool = False):
+                 scene_mesh: Optional[SceneMesh] = None, esdf: bool = False, esdf_camera_margin: int = 0):
+        if esdf_camera_margin and not esdf:
+            raise ValueError("DepthmapNode: esdf_camera_margin needs esdf=True")
+        if int(esdf_camera_margin) != esdf_camera_margin or esdf_camera_margin < 0:
+            raise ValueError("DepthmapNode: esdf_camera_margin must be a whole number of voxels >= 0")
         if prior_from_volume and volume is None:
             raise ValueError("DepthmapNode: prior_from_volume needs a volume")
         if follow_volume and volume is None:
@@ -58,6 +73,9 @@ class DepthmapNode:
         # when set, the volume's ESDF is recomputed after each keyframe is fused and published as ("volume_esdf",
         # volume), ready for esdfQuery
         self.esdf_ = bool(esdf)
+        # when > 0, that ESDF covers the bounding box of the window and the cube of this half-side (voxels) around the
+        # finished keyframe's camera, so that the camera -- outside a following window -- can query it
+        self.esdf_camera_margin_ = int(esdf_camera_margin)
         self.ref_depth_range_ = (0.0, 0.0)   # [min_depth, max_depth] of the current keyframe
         self.state_ = TAKE_REFERENCE_FRAME                      # src/depthmap_node.cpp:35
         self.ref_compl_perc_ = float(ref_compl_perc)            # :81, default 10.0
@@ -100,9 +118,21 @@ class DepthmapNode:
         if self.publisher_:
             self.publisher_("depthmap_and_pointcloud", self.depthmap_)
         if self.esdf_:
-            self.volume_.computeEsdf()
+            if self.esdf_camera_margin_:
+                self.volume_.computeEsdf(*self.esdfCameraBox())
+            else:
+                self.volume_.computeEsdf()
             if self.publisher_:
                 self.publisher_("volume_esdf", self.volume_)
+
+    def esdfCameraBox(self):
+        """(lo int64 [3], dims int64 [3]) in window indices: the bounding box of the window and of the cube of
+        half-side esdf_camera_margin voxels around the finished keyframe's camera centre, which followVolume's
+        conversion to window indices places at round((centre - origin) / voxel_size)."""
+        v = self.volume_
+        T = np.asarray(self.depthmap_.getT_world_ref().data, np.float64).reshape(3, 4)
+        return esdf_camera_box(v.dims, v.voxel_size, v.origin, T[:, 3], self.esdf_camera_margin_)
+
 
     def followVolume(self) -> None:
         """Recentre volume_ on the finished keyframe's view centre -- the camera centre plus the middle of
