@@ -84,6 +84,16 @@ public:
                                               T_curr_world.data.data, dev_depth, depth_pitch),
                            "TsdfVolume: unable to raycast");
   }
+  // The same rays through a box of the map instead of the window: lower corner lo (window indices, may lie outside
+  // the window) and dims; each box voxel takes the window's record, else its stored brick's, else unknown, as
+  // computeEsdf(lo, dims) gathers them (rmd_volume_raycast_box).  8 B of scratch per box voxel.
+  void raycast(int width, int height, const PinholeCamera &cam, const SE3<float> &T_curr_world, float *dev_depth,
+               size_t depth_pitch, const int64_t lo[3], const int dims[3])
+  {
+    detail::throw_on_error(rmd_volume_raycast_box(handle_, lo, dims, width, height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                                  T_curr_world.data.data, dev_depth, depth_pitch, NULL, 0, NULL, 0),
+                           "TsdfVolume: unable to raycast a box");
+  }
 
   // Right after seeds.setReferenceImage (no update since): the new keyframe's depth prior from the fused model --
   // every non-BORDER pixel whose ray hits the surface within the seeds' depth range gets (hit, sigma_sq_frac *
@@ -93,6 +103,12 @@ public:
   {
     detail::throw_on_error(rmd_volume_prior_seeds(handle_, seeds.handle(), sigma_sq_frac),
                            "TsdfVolume: unable to seed the keyframe prior");
+  }
+  // The same from a box of the map (rmd_volume_prior_seeds_box), e.g. the box around the keyframe's view.
+  void seedPrior(SeedMatrix &seeds, float sigma_sq_frac, const int64_t lo[3], const int dims[3])
+  {
+    detail::throw_on_error(rmd_volume_prior_seeds_box(handle_, seeds.handle(), sigma_sq_frac, lo, dims),
+                           "TsdfVolume: unable to seed the keyframe prior from a box");
   }
 
   // Intensity channel (8 B per voxel): from now on integrate() also fuses the keyframe's reference image.
@@ -135,6 +151,16 @@ public:
                                                         dev_intensity, intensity_pitch),
                            "TsdfVolume: unable to raycast the intensity");
   }
+  // raycastIntensity() through a box of the map, as raycast(..., lo, dims); 8 B more per box voxel.
+  void raycastIntensity(int width, int height, const PinholeCamera &cam, const SE3<float> &T_curr_world,
+                        float *dev_depth, size_t depth_pitch, float *dev_intensity, size_t intensity_pitch,
+                        const int64_t lo[3], const int dims[3])
+  {
+    detail::throw_on_error(rmd_volume_raycast_box(handle_, lo, dims, width, height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                                  T_curr_world.data.data, dev_depth, depth_pitch, dev_intensity,
+                                                  intensity_pitch, NULL, 0),
+                           "TsdfVolume: unable to raycast the intensity of a box");
+  }
 
   // One unit normal (nx, ny, nz, 0) per surface point (= mesh vertex), in surfacePoints() order, towards free space;
   // (0, 0, 0, 0) where the tsdf gradient vanishes.
@@ -159,6 +185,16 @@ public:
                                                       T_curr_world.data.data, dev_depth, depth_pitch, dev_normals,
                                                       normals_pitch),
                            "TsdfVolume: unable to raycast the normals");
+  }
+  // raycastNormals() through a box of the map, as raycast(..., lo, dims).
+  void raycastNormals(int width, int height, const PinholeCamera &cam, const SE3<float> &T_curr_world,
+                      float *dev_depth, size_t depth_pitch, float *dev_normals, size_t normals_pitch,
+                      const int64_t lo[3], const int dims[3])
+  {
+    detail::throw_on_error(rmd_volume_raycast_box(handle_, lo, dims, width, height, cam.fx, cam.fy, cam.cx, cam.cy,
+                                                  T_curr_world.data.data, dev_depth, depth_pitch, NULL, 0, dev_normals,
+                                                  normals_pitch),
+                           "TsdfVolume: unable to raycast the normals of a box");
   }
 
   // Moving volume: voxel (i, j, k) then holds what (i + dx, j + dy, k + dz) held (unknown outside the grid), and the

@@ -831,6 +831,42 @@ int rmd_volume_esdf_box(rmd_volume_t *v, const int64_t lo[3], const int dims[3])
  * Any output may be NULL.  RMD_ERR_NOT_INITIALISED before the first
  * compute. */
 int rmd_volume_esdf_info(rmd_volume_t *v, int64_t lo_unbounded[3], int dims[3], float origin[3]);
+/* Raycasts of a box of the map (DESIGN.md 4.8), so that a following volume
+ * renders, and seeds its keyframe prior from, the surface it has already
+ * mapped in front of and beyond the window.  The box (lo, dims), its records
+ * (window, else stored brick, else (0, 0); intensity records likewise from
+ * the channel's window and store) and its origin are rmd_volume_esdf_box's.
+ *   rmd_volume_raycast_box: exactly what rmd_volume_raycast,
+ * rmd_volume_raycast_intensity or rmd_volume_raycast_normals return on a grid
+ * of dims m at the box's origin holding the box's records: the same slab
+ * clip, samples, hit rule and outputs.  The box (0, n) gives the window's
+ * images bit for bit.  dev_intensity and dev_normals may each be NULL; with
+ * both, dev_depth is written twice with the same bits.  Asynchronous on the
+ * volume's stream.
+ *   rmd_volume_prior_seeds_box: rmd_volume_prior_seeds on the box's records:
+ * BORDER pixels are skipped, a hit d with min_depth <= d <= max_depth becomes
+ * (d, sigma_sq_frac * range^2 / 36, 10, 10), every other seed is left as it
+ * is.  Its preconditions and error codes are rmd_volume_prior_seeds'.  No host
+ * synchronisation: the records are gathered on the volume's stream, the rays
+ * run on s's stream after them, and the volume's stream waits for the rays, so
+ * a later shift, integrate, upload, ESDF or box call cannot overwrite what
+ * they read.
+ *   Memory: 8 B per box voxel of gathered records, 8 B more with intensity,
+ * and with a non-empty store 4 B per brick of the box for the brick table;
+ * scratch shared with rmd_volume_esdf_box, grown on demand, new buffers
+ * allocated before old ones are freed, so a failure
+ * (cudaErrorMemoryAllocation, also for records larger than the device) leaves
+ * the window, the store and the ESDF snapshot as they were.
+ *   RMD_ERR_INVALID_ARGUMENT: null handle or pointer, a dimension <= 0,
+ * D + lo + m overflowing int64, rmd_volume_raycast*'s pitch and alignment
+ * rules.  RMD_ERR_UNSUPPORTED: a dimension > 65535.  RMD_ERR_NOT_INITIALISED:
+ * intensity asked of a volume without the channel. */
+int rmd_volume_raycast_box(rmd_volume_t *v, const int64_t lo[3], const int dims[3], int width, int height, float fx,
+                           float fy, float cx, float cy, const float *T_curr_world, float *dev_depth,
+                           size_t depth_pitch, float *dev_intensity, size_t intensity_pitch, float *dev_normals,
+                           size_t normals_pitch);
+int rmd_volume_prior_seeds_box(rmd_volume_t *v, rmd_seeds_t *s, float sigma_sq_frac, const int64_t lo[3],
+                               const int dims[3]);
 /* Test / checkpoint hook (like rmd_volume_download): the snapshot's distance
  * and weight, one float each per voxel of the snapshot (mx * my * mz, the
  * window's nx * ny * nz for rmd_volume_esdf), x fastest.  Synchronous. */

@@ -113,6 +113,8 @@ _SIGNATURES = {
     "rmd_volume_esdf": (ci, [vp]),
     "rmd_volume_esdf_box": (ci, [vp, vp, vp]),
     "rmd_volume_esdf_info": (ci, [vp, vp, vp, vp]),
+    "rmd_volume_raycast_box": (ci, [vp, vp, vp, ci, ci, cf, cf, cf, cf, vp, vp, cs, vp, cs, vp, cs]),
+    "rmd_volume_prior_seeds_box": (ci, [vp, vp, cf, vp, vp]),
     "rmd_volume_download_esdf": (ci, [vp, vp, vp]),
     "rmd_volume_esdf_query": (ci, [vp, vp, cs, vp, vp]),
     "rmd_volume_esdf_query_device": (ci, [vp, vp, cs, vp, vp]),

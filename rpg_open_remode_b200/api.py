@@ -138,6 +138,20 @@ class SE3:
         return "SE3(\n%s)" % self.data.reshape(3, 4)
 
 
+def _box_args(lo, dims, what: str):
+    """None when lo and dims are both omitted, else (lo int64 [3], dims int32 [3]) of a box of a volume's map."""
+    if lo is None and dims is None:
+        return None
+    if lo is None or dims is None:
+        raise ValueError(what + ": lo and dims come together")
+    a, m = list(np.asarray(lo).reshape(-1)), list(np.asarray(dims).reshape(-1))
+    if len(a) != 3 or len(m) != 3 or any(int(x) != x for x in a + m):
+        raise ValueError(what + ": lo and dims must be three whole numbers each")
+    if any(not -2 ** 63 <= int(x) < 2 ** 63 for x in a) or any(not -2 ** 31 <= int(x) < 2 ** 31 for x in m):
+        raise ValueError(what + ": lo must fit int64 and dims int32")
+    return np.array([int(x) for x in a], np.int64), np.array([int(x) for x in m], np.int32)
+
+
 def _pose12(T) -> np.ndarray:
     if isinstance(T, SE3):
         return np.ascontiguousarray(T.data, dtype=_f32)
@@ -213,6 +227,7 @@ class SeedMatrix:
 
     def __init__(self, width, height, cam: PinholeCamera, patch_side=5, device=-1):
         self.width_, self.height_, self.patch_side = int(width), int(height), int(patch_side)
+        self.cam_ = cam
         self._L = _native.lib()
         h = ctypes.c_void_p()
         check(self._L.rmd_seeds_create(self.width_, self.height_, cam.fx, cam.fy, cam.cx, cam.cy,
@@ -381,13 +396,21 @@ class SeedMatrix:
         check(self._L.rmd_seeds_propagate_prior(self._h, src.handle, float(sigma_sq_frac)),
               "SeedMatrix::propagatePriorFrom")
 
-    def priorFromVolume(self, volume: "TsdfVolume", sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC) -> None:
+    def priorFromVolume(self, volume: "TsdfVolume", sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC, lo=None,
+                        dims=None) -> None:
         """Right after setReferenceImage* (no update since): every pixel whose ray from the new reference pose hits
         the fused surface of `volume` within [min_depth, max_depth] takes the hit as its depth prior (sigma^2 =
         sigma_sq_frac * range^2 / 36); all other seeds keep the prior they have (uniform, or splatted by the
-        propagation above).  Ordered on the device after the volume's queued integrations."""
-        check(self._L.rmd_volume_prior_seeds(volume.handle, self._h, float(sigma_sq_frac)),
-              "SeedMatrix::priorFromVolume")
+        propagation above).  Ordered on the device after the volume's queued integrations.  lo, dims: the rays
+        march that box of the map instead of the window, brick store included (TsdfVolume.raycast)."""
+        what = "SeedMatrix::priorFromVolume"
+        box = _box_args(lo, dims, what)
+        if box is None:
+            check(self._L.rmd_volume_prior_seeds(volume.handle, self._h, float(sigma_sq_frac)), what)
+            return
+        lo64, m32 = box
+        check(self._L.rmd_volume_prior_seeds_box(volume.handle, self._h, float(sigma_sq_frac), lo64.ctypes.data,
+                                                 m32.ctypes.data), what)
 
     def uploadState(self, field: int, values) -> None:
         dt = np.int32 if field == FIELD_CONVERGENCE else np.float32
@@ -639,35 +662,67 @@ class TsdfVolume:
                                       ctypes.byref(nv), ctypes.byref(nt)), "TsdfVolume::mesh")
         return verts[:min(int(vertex_capacity), nv.value)], tris[:min(int(triangle_capacity), nt.value)]
 
-    def raycast(self, cam: PinholeCamera, T_curr_world, width: int, height: int) -> np.ndarray:
-        """float32 [height, width]: distance along each pixel's ray to the fused surface, 0 where none."""
+    def _raycast_box(self, what, box, cam, T, width, height, img, inten=None, nrm=None) -> None:
+        lo64, m32 = box
+        check(self._L.rmd_volume_raycast_box(self._h, lo64.ctypes.data, m32.ctypes.data, int(width), int(height),
+                                             cam.fx, cam.fy, cam.cx, cam.cy, T.ctypes.data, img.data, img.pitch,
+                                             inten.data if inten is not None else None,
+                                             inten.pitch if inten is not None else 0,
+                                             nrm.data if nrm is not None else None,
+                                             nrm.pitch if nrm is not None else 0), what)
+
+    def raycast(self, cam: PinholeCamera, T_curr_world, width: int, height: int, lo=None, dims=None) -> np.ndarray:
+        """float32 [height, width]: distance along each pixel's ray to the fused surface, 0 where none.
+
+        With lo (int [3], window indices, may be negative or outside the window) and dims (int [3], each > 0): the
+        rays march a box of the map instead of the window -- each box voxel takes the window's record, else (with the
+        store) its stored brick's, else unknown, as computeEsdf(lo, dims) gathers them.  8 B of scratch per box
+        voxel; the box (0, n) gives the window's image bit for bit."""
+        what = "TsdfVolume::raycast"
+        box = _box_args(lo, dims, what)
         img = DeviceImage(width, height, "float32")
         T = _pose12(T_curr_world)
+        if box is not None:
+            self._raycast_box(what, box, cam, T, width, height, img)
+            self.sync()
+            return img.getDevData()
         check(self._L.rmd_volume_raycast(self._h, int(width), int(height), cam.fx, cam.fy, cam.cx, cam.cy,
                                          T.ctypes.data, img.data, img.pitch), "TsdfVolume::raycast")
         self.sync()
         return img.getDevData()
 
-    def raycastIntensity(self, cam: PinholeCamera, T_curr_world, width: int, height: int):
+    def raycastIntensity(self, cam: PinholeCamera, T_curr_world, width: int, height: int, lo=None, dims=None):
         """(depth, intensity), float32 [height, width] each: raycast()'s depth, bit for bit, and the fused intensity
-        at each hit, -1 where there is no hit or no intensity."""
+        at each hit, -1 where there is no hit or no intensity.  lo, dims: a box of the map, as raycast(); 8 B more
+        per box voxel for its intensity records."""
+        what = "TsdfVolume::raycastIntensity"
+        box = _box_args(lo, dims, what)
         img, inten = DeviceImage(width, height, "float32"), DeviceImage(width, height, "float32")
         T = _pose12(T_curr_world)
+        if box is not None:
+            self._raycast_box(what, box, cam, T, width, height, img, inten=inten)
+            self.sync()
+            return img.getDevData(), inten.getDevData()
         check(self._L.rmd_volume_raycast_intensity(self._h, int(width), int(height), cam.fx, cam.fy, cam.cx, cam.cy,
                                                    T.ctypes.data, img.data, img.pitch, inten.data, inten.pitch),
               "TsdfVolume::raycastIntensity")
         self.sync()
         return img.getDevData(), inten.getDevData()
 
-    def raycastNormals(self, cam: PinholeCamera, T_curr_world, width: int, height: int):
+    def raycastNormals(self, cam: PinholeCamera, T_curr_world, width: int, height: int, lo=None, dims=None):
         """(depth float32 [height, width], normals float32 [height, width, 3]): raycast()'s depth, bit for bit, and
         the world-frame unit normal of the fused surface at each hit, (0, 0, 0) where there is no hit or no
-        normal."""
+        normal.  lo, dims: a box of the map, as raycast()."""
+        what = "TsdfVolume::raycastNormals"
+        box = _box_args(lo, dims, what)
         img, nrm = DeviceImage(width, height, "float32"), DeviceImage(4 * int(width), height, "float32")
         T = _pose12(T_curr_world)
-        check(self._L.rmd_volume_raycast_normals(self._h, int(width), int(height), cam.fx, cam.fy, cam.cx, cam.cy,
-                                                 T.ctypes.data, img.data, img.pitch, nrm.data, nrm.pitch),
-              "TsdfVolume::raycastNormals")
+        if box is not None:
+            self._raycast_box(what, box, cam, T, width, height, img, nrm=nrm)
+        else:
+            check(self._L.rmd_volume_raycast_normals(self._h, int(width), int(height), cam.fx, cam.fy, cam.cx,
+                                                     cam.cy, T.ctypes.data, img.data, img.pitch, nrm.data, nrm.pitch),
+                  what)
         self.sync()
         return img.getDevData(), np.ascontiguousarray(nrm.getDevData().reshape(int(height), int(width), 4)[..., :3])
 
@@ -883,19 +938,12 @@ class TsdfVolume:
         brick's, else unknown; the snapshot's origin is origin + lo * voxel_size from the creation origin and the
         total offset, so esdfQuery answers around the box and obstacles in the store count.  24 B per box voxel.
         esdfBox() tells which box the snapshot answers for."""
-        if lo is None and dims is None:
-            check(self._L.rmd_volume_esdf(self._h), "TsdfVolume::computeEsdf")
-            return
         what = "TsdfVolume::computeEsdf"
-        if lo is None or dims is None:
-            raise ValueError(what + ": lo and dims come together")
-        a, m = list(np.asarray(lo).reshape(-1)), list(np.asarray(dims).reshape(-1))
-        if len(a) != 3 or len(m) != 3 or any(int(x) != x for x in a + m):
-            raise ValueError(what + ": lo and dims must be three whole numbers each")
-        if any(not -2 ** 63 <= int(x) < 2 ** 63 for x in a) or any(not -2 ** 31 <= int(x) < 2 ** 31 for x in m):
-            raise ValueError(what + ": lo must fit int64 and dims int32")
-        lo64 = np.array([int(x) for x in a], np.int64)
-        m32 = np.array([int(x) for x in m], np.int32)
+        box = _box_args(lo, dims, what)
+        if box is None:
+            check(self._L.rmd_volume_esdf(self._h), what)
+            return
+        lo64, m32 = box
         check(self._L.rmd_volume_esdf_box(self._h, lo64.ctypes.data, m32.ctypes.data), what)
 
     def esdfBox(self):
@@ -1175,10 +1223,11 @@ class Depthmap:
         (SeedMatrix.setPriorPropagation); 0 switches it off (the default of a new Depthmap)."""
         self.seeds_.setPriorPropagation(sigma_sq_frac)
 
-    def priorFromVolume(self, volume: TsdfVolume, sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC) -> None:
-        """After setReferenceImage: the new keyframe's depth prior from the model fused so far
-        (SeedMatrix.priorFromVolume)."""
-        self.seeds_.priorFromVolume(volume, sigma_sq_frac)
+    def priorFromVolume(self, volume: TsdfVolume, sigma_sq_frac: float = PRIOR_SIGMA_SQ_FRAC, lo=None,
+                        dims=None) -> None:
+        """After setReferenceImage: the new keyframe's depth prior from the model fused so far, or with lo and dims
+        from that box of the map (SeedMatrix.priorFromVolume)."""
+        self.seeds_.priorFromVolume(volume, sigma_sq_frac, lo, dims)
 
     def update(self, img_curr, T_curr_world) -> None:
         self.seeds_.update(self._input_image(img_curr), T_curr_world)

@@ -2144,15 +2144,28 @@ int rmd_volume_integrate_seeds(rmd_volume_t *v, rmd_seeds_t *s, const float *dev
   return 0;
 }
 
-int rmd_volume_prior_seeds(rmd_volume_t *v, rmd_seeds_t *s, float sigma_sq_frac)
+} // extern "C"
+
+namespace
 {
-  RMD_REQUIRE(v && s, "rmd_volume_prior_seeds: null handle");
-  RMD_REQUIRE(v->device == s->device, "rmd_volume_prior_seeds: volume and seeds on different devices");
-  RMD_REQUIRE(sigma_sq_frac > 0.0f && sigma_sq_frac <= 1.0f, "rmd_volume_prior_seeds: sigma_sq_frac must be in (0, 1]");
+
+// rmd_volume_prior_seeds[_box]: box, the box (lo, dims) of the map instead of the window.
+int volume_prior_seeds(const char *what, rmd_volume_t *v, rmd_seeds_t *s, float sigma_sq_frac, bool box,
+                       const int64_t lo[3], const int dims[3])
+{
+  const std::string w(what);
+  RMD_REQUIRE(v && s, (w + ": null handle").c_str());
+  RMD_REQUIRE(v->device == s->device, (w + ": volume and seeds on different devices").c_str());
+  RMD_REQUIRE(sigma_sq_frac > 0.0f && sigma_sq_frac <= 1.0f, (w + ": sigma_sq_frac must be in (0, 1]").c_str());
   if(!s->has_reference || s->frame_index != 0)
-    return fail(RMD_ERR_NOT_INITIALISED,
-                "rmd_volume_prior_seeds: the seeds need a reference frame set since their last update");
+    return fail(RMD_ERR_NOT_INITIALISED, (w + ": the seeds need a reference frame set since their last update").c_str());
   DeviceGuard guard(s->device);
+  VolumeGrid g = v->g;
+  if(box)   // the box's records, gathered on the volume's stream: the hand-off below orders the rays after them
+  {
+    const int rc = volume_box_records(v, lo, dims, g, NULL, what);
+    if(rc) return rc;
+  }
   {
     const int rc = wait_external(s);
     if(rc) return rc;
@@ -2163,7 +2176,7 @@ int rmd_volume_prior_seeds(rmd_volume_t *v, rmd_seeds_t *s, float sigma_sq_frac)
   RMD_CUDA_TRY(cudaStreamWaitEvent(s->stream, v->seeds_ev, 0));
   VolumeRaycastParams P;
   memset(&P, 0, sizeof(P));
-  P.g = v->g;
+  P.g = g;
   P.width = s->width; P.height = s->height;
   P.cam = s->cam;
   P.T_world_curr = s->T_world_ref;   // = pose_inverse(pose_from(T_curr_world)), as rmd_volume_raycast computes it
@@ -2175,11 +2188,28 @@ int rmd_volume_prior_seeds(rmd_volume_t *v, rmd_seeds_t *s, float sigma_sq_frac)
   S.sigma_sq = sigma_sq_frac * s->sigma_sq_max;   // as prior_apply
   RMD_CUDA_TRY(launch_volume_prior(P, S, s->stream));
   s->n_total += 1;
-  // ... and a later writer of the volume (integrate, reset, upload) waits for the rays' reads.  The wait above has
-  // already taken the event's previous record, so recording it again loses nothing.
+  // ... and a later writer of the volume (integrate, reset, upload; for a box also the next gather into the same
+  // scratch) waits for the rays' reads.  The wait above has already taken the event's previous record, so recording
+  // it again loses nothing.
   RMD_CUDA_TRY(cudaEventRecord(v->seeds_ev, s->stream));
   RMD_CUDA_TRY(cudaStreamWaitEvent(v->stream, v->seeds_ev, 0));
   return 0;
+}
+
+} // namespace
+
+extern "C"
+{
+
+int rmd_volume_prior_seeds(rmd_volume_t *v, rmd_seeds_t *s, float sigma_sq_frac)
+{
+  return volume_prior_seeds("rmd_volume_prior_seeds", v, s, sigma_sq_frac, false, NULL, NULL);
+}
+
+int rmd_volume_prior_seeds_box(rmd_volume_t *v, rmd_seeds_t *s, float sigma_sq_frac, const int64_t lo[3],
+                               const int dims[3])
+{
+  return volume_prior_seeds("rmd_volume_prior_seeds_box", v, s, sigma_sq_frac, true, lo, dims);
 }
 
 } // extern "C"

@@ -644,22 +644,25 @@ float shifted_origin(float origin, long long D, float s)
   return origin + step;
 }
 
-// The ESDF buffers for a snapshot of n voxels, with the gathered records of a box (records) and a brick table of
-// `table` entries (0: none).  Every new buffer is allocated before any old one is freed, so that a failure leaves the
-// previous snapshot as it was; a snapshot whose buffer is replaced is gone until the compute that follows.
-int esdf_reserve(rmd_volume *v, size_t n, bool records, size_t table, const char *what)
+// The ESDF and box buffers: a snapshot of n voxels (0: none), the gathered records of a box of `records` voxels, its
+// gathered intensity records of `colour` voxels and a brick table of `table` entries (0: none needed).  Every new
+// buffer is allocated before any old one is freed, so that a failure leaves the previous snapshot as it was; a
+// snapshot whose buffer is replaced is gone until the compute that follows.
+int box_reserve(rmd_volume *v, size_t n, size_t records, size_t colour, size_t table, const char *what)
 {
-  const bool grow = n > v->esdf_cap, grow_rec = records && n > v->esdf_rec_cap, grow_table = table > v->esdf_table_cap;
-  float2 *e = NULL, *r = NULL;
+  const bool grow = n > v->esdf_cap, grow_rec = records > v->esdf_rec_cap, grow_col = colour > v->box_col_cap,
+             grow_table = table > v->esdf_table_cap;
+  float2 *e = NULL, *r = NULL, *c = NULL;
   int *s = NULL, *t = NULL;
   cudaError_t err = cudaSuccess;
   if(grow) err = cudaMalloc(&e, sizeof(float2) * n);
   if(err == cudaSuccess && grow) err = cudaMalloc(&s, 2 * sizeof(int) * n);
-  if(err == cudaSuccess && grow_rec) err = cudaMalloc(&r, sizeof(float2) * n);
+  if(err == cudaSuccess && grow_rec) err = cudaMalloc(&r, sizeof(float2) * records);
+  if(err == cudaSuccess && grow_col) err = cudaMalloc(&c, sizeof(float2) * colour);
   if(err == cudaSuccess && grow_table) err = cudaMalloc(&t, sizeof(int) * table);
   if(err != cudaSuccess)
   {
-    cudaFree(e); cudaFree(s); cudaFree(r); cudaFree(t);
+    cudaFree(e); cudaFree(s); cudaFree(r); cudaFree(c); cudaFree(t);
     cudaGetLastError();
     return fail_cuda(err, what);
   }
@@ -672,7 +675,12 @@ int esdf_reserve(rmd_volume *v, size_t n, bool records, size_t table, const char
   if(grow_rec)
   {
     cudaFree(v->esdf_rec);
-    v->esdf_rec = r; v->esdf_rec_cap = n;
+    v->esdf_rec = r; v->esdf_rec_cap = records;
+  }
+  if(grow_col)
+  {
+    cudaFree(v->box_col);
+    v->box_col = c; v->box_col_cap = colour;
   }
   if(grow_table)
   {
@@ -712,7 +720,109 @@ int esdf_passes(rmd_volume *v, const VolumeGrid &g, const long long lo[3], const
   return 0;
 }
 
+// The records of the box (lo, dims) -- its unbounded voxels [base, base + dims) -- gathered into v->esdf_rec, and with
+// col its intensity records into v->box_col (DESIGN.md 4.8), with the buffers grown for them and, with n_snapshot > 0,
+// for an ESDF snapshot of that many voxels.  B: the box's grid on the gathered records.  Asynchronous on v's stream.
+int box_gather(rmd_volume *v, const int64_t lo[3], const int dims[3], const long long base[3], size_t n_snapshot,
+               VolumeGrid &B, const float2 **col, const char *what)
+{
+  const int n[3] = {v->g.nx, v->g.ny, v->g.nz};
+  VolumeEsdfGatherParams G;
+  memset(&G, 0, sizeof(G));
+  G.g = v->g;
+  G.mx = dims[0]; G.my = dims[1]; G.mz = dims[2];
+  // the window's part, box index i = window index - lo: [max(0, -lo), min(m, n - lo)) when lo lies in (-m, n)
+  bool meets = true, inside = true;
+  for(int a = 0; a < 3; ++a)
+    meets = meets && lo[a] < n[a] && lo[a] > -(long long)dims[a];
+  for(int a = 0; meets && a < 3; ++a)
+  {
+    const int l = (int)lo[a];
+    const long long h = (long long)n[a] - l;
+    G.wlo[a] = l < 0 ? -l : 0;
+    G.whi[a] = h < dims[a] ? (int)h : dims[a];
+    G.wof[a] = l;
+    inside = inside && G.wlo[a] == 0 && G.whi[a] == dims[a];
+  }
+  inside = meets && inside;
+  // the brick table over the box's bricks [floor(base / 8), floor((base + dims - 1) / 8)]
+  std::vector<int> table;
+  const bool lookup = v->store && !v->store->index.slot.empty() && !inside;
+  if(lookup)
+  {
+    int64_t b0[3];
+    int nb[3];
+    for(int a = 0; a < 3; ++a)
+    {
+      b0[a] = brick_floor(base[a]);
+      nb[a] = (int)(brick_floor(base[a] + dims[a] - 1) - b0[a] + 1);
+      G.r[a] = (int)(base[a] - b0[a] * STORE_BRICK);
+      G.tb[a] = nb[a];
+    }
+    table = store_brick_table(v->store->index, b0, nb);
+  }
+  DeviceGuard guard(v->device);
+  const size_t m = (size_t)dims[0] * (size_t)dims[1] * (size_t)dims[2];
+  int rc = box_reserve(v, n_snapshot, m, col ? m : 0, table.size(), what);
+  if(rc) return rc;
+  if(lookup)
+  {
+    // pageable source: the copy is staged before the call returns
+    RMD_CUDA_TRY(cudaMemcpyAsync(v->esdf_table, table.data(), sizeof(int) * table.size(), cudaMemcpyHostToDevice,
+                                 v->stream));
+    G.table = v->esdf_table;
+    G.pool = v->store->pool;
+  }
+  G.out = v->esdf_rec;
+  RMD_CUDA_TRY(launch_volume_esdf_gather(G, v->stream));
+  if(col)   // the intensity records by the same rule, from the colour window and pool_col
+  {
+    G.g.vox = v->col;
+    if(lookup) G.pool = v->store->pool_col;
+    G.out = v->box_col;
+    RMD_CUDA_TRY(launch_volume_esdf_gather(G, v->stream));
+    *col = v->box_col;
+  }
+  B = v->g;
+  B.vox = v->esdf_rec;
+  B.nx = dims[0]; B.ny = dims[1]; B.nz = dims[2];
+  const float og[3] = {v->g.ox, v->g.oy, v->g.oz};
+  float o[3];
+  for(int a = 0; a < 3; ++a)   // lo = 0: the window's origin itself
+    o[a] = lo[a] == 0 ? og[a] : shifted_origin(v->o0[a], base[a], v->g.voxel);
+  B.ox = o[0]; B.oy = o[1]; B.oz = o[2];
+  return 0;
+}
+
 } // namespace
+
+namespace rmdb
+{
+
+int volume_box_records(rmd_volume *v, const int64_t lo[3], const int dims[3], VolumeGrid &B, const float2 **col,
+                       const char *what)
+{
+  VOLUME_REQUIRE(v && lo && dims, "null argument");
+  VOLUME_REQUIRE(dims[0] > 0 && dims[1] > 0 && dims[2] > 0, "box dimensions must be positive");
+  long long base[3], end[3];   // the box's unbounded voxels [D + lo, D + lo + dims)
+  for(int a = 0; a < 3; ++a)
+    VOLUME_REQUIRE(!__builtin_add_overflow(v->D[a], (long long)lo[a], &base[a]) &&
+                   !__builtin_add_overflow(base[a], (long long)dims[a], &end[a]),
+                   "the total offset plus the box's corner and size overflows");
+  // the gather's grid is (ceil(mx / 128), my, mz) blocks
+  if(dims[0] > 65535 || dims[1] > 65535 || dims[2] > 65535)
+    return fail(RMD_ERR_UNSUPPORTED, (std::string(what) + ": box dimensions must be <= 65535").c_str());
+  DeviceGuard guard(v->device);
+  // refused before the host builds a brick table for a box whose records could never be allocated
+  size_t free_bytes = 0, total_bytes = 0;
+  RMD_CUDA_TRY(cudaMemGetInfo(&free_bytes, &total_bytes));
+  const size_t m = (size_t)dims[0] * (size_t)dims[1] * (size_t)dims[2];
+  if(m > total_bytes / (sizeof(float2) * (col ? 2 : 1)))
+    return fail((int)cudaErrorMemoryAllocation, (std::string(what) + ": the box's records exceed the device").c_str());
+  return box_gather(v, lo, dims, base, 0, B, col, what);
+}
+
+} // namespace rmdb
 
 extern "C"
 {
@@ -776,7 +886,7 @@ int rmd_volume_destroy(rmd_volume_t *v)
     cudaFree(v->store->bricks); cudaFree(v->store->flags);
     delete v->store;
   }
-  cudaFree(v->esdf); cudaFree(v->esdf_scratch); cudaFree(v->esdf_rec); cudaFree(v->esdf_table);
+  cudaFree(v->esdf); cudaFree(v->esdf_scratch); cudaFree(v->esdf_rec); cudaFree(v->esdf_table); cudaFree(v->box_col);
   cudaGetLastError();
   delete v;
   return 0;
@@ -1285,7 +1395,7 @@ int rmd_volume_esdf(rmd_volume_t *v)
     return fail(RMD_ERR_UNSUPPORTED, "rmd_volume_esdf: (nx-1)^2 + (ny-1)^2 + (nz-1)^2 must be < 2^24");
   DeviceGuard guard(v->device);
   // the window's records as they are: no gather
-  const int rc = esdf_reserve(v, v->n_vox, false, 0, what);
+  const int rc = box_reserve(v, v->n_vox, 0, 0, 0, what);
   if(rc) return rc;
   const float o[3] = {v->g.ox, v->g.oy, v->g.oz};
   return esdf_passes(v, v->g, v->D, o);
@@ -1296,7 +1406,6 @@ int rmd_volume_esdf_box(rmd_volume_t *v, const int64_t lo[3], const int dims[3])
   const char *what = "rmd_volume_esdf_box";
   VOLUME_REQUIRE(v && lo && dims, "null argument");
   VOLUME_REQUIRE(dims[0] > 0 && dims[1] > 0 && dims[2] > 0, "box dimensions must be positive");
-  const int n[3] = {v->g.nx, v->g.ny, v->g.nz};
   long long base[3], end[3];   // the box's unbounded voxels [D + lo, D + lo + dims)
   for(int a = 0; a < 3; ++a)
     VOLUME_REQUIRE(!__builtin_add_overflow(v->D[a], (long long)lo[a], &base[a]) &&
@@ -1305,63 +1414,58 @@ int rmd_volume_esdf_box(rmd_volume_t *v, const int64_t lo[3], const int dims[3])
   const long long ex = dims[0] - 1, ey = dims[1] - 1, ez = dims[2] - 1;
   if(ex * ex + ey * ey + ez * ez >= (1ll << 24))
     return fail(RMD_ERR_UNSUPPORTED, "rmd_volume_esdf_box: (mx-1)^2 + (my-1)^2 + (mz-1)^2 must be < 2^24");
-  VolumeEsdfGatherParams G;
-  memset(&G, 0, sizeof(G));
-  G.g = v->g;
-  G.mx = dims[0]; G.my = dims[1]; G.mz = dims[2];
-  // the window's part, box index i = window index - lo: [max(0, -lo), min(m, n - lo)) when lo lies in (-m, n)
-  bool meets = true, inside = true;
-  for(int a = 0; a < 3; ++a)
-    meets = meets && lo[a] < n[a] && lo[a] > -(long long)dims[a];
-  for(int a = 0; meets && a < 3; ++a)
+  const size_t m = (size_t)dims[0] * (size_t)dims[1] * (size_t)dims[2];
+  VolumeGrid B;
+  const int rc = box_gather(v, lo, dims, base, m, B, NULL, what);
+  if(rc) return rc;
+  const float o[3] = {B.ox, B.oy, B.oz};
+  return esdf_passes(v, B, base, o);
+}
+
+int rmd_volume_raycast_box(rmd_volume_t *v, const int64_t lo[3], const int dims[3], int width, int height, float fx,
+                           float fy, float cx, float cy, const float *T_curr_world, float *dev_depth,
+                           size_t depth_pitch, float *dev_intensity, size_t intensity_pitch, float *dev_normals,
+                           size_t normals_pitch)
+{
+  const char *what = "rmd_volume_raycast_box";
+  VOLUME_REQUIRE(v && T_curr_world && dev_depth, "null argument");
+  VOLUME_REQUIRE(width > 0 && height > 0, "bad image size");
+  VOLUME_REQUIRE(depth_pitch_ok(depth_pitch, width), "bad depth pitch");
+  if(dev_intensity)
   {
-    const int l = (int)lo[a];
-    const long long h = (long long)n[a] - l;
-    G.wlo[a] = l < 0 ? -l : 0;
-    G.whi[a] = h < dims[a] ? (int)h : dims[a];
-    G.wof[a] = l;
-    inside = inside && G.wlo[a] == 0 && G.whi[a] == dims[a];
+    VOLUME_REQUIRE(depth_pitch_ok(intensity_pitch, width), "bad intensity pitch");
+    if(!v->col)
+      return no_intensity(what);
   }
-  inside = meets && inside;
-  // the brick table over the box's bricks [floor(base / 8), floor((end - 1) / 8)]
-  std::vector<int> table;
-  const bool lookup = v->store && !v->store->index.slot.empty() && !inside;
-  if(lookup)
+  if(dev_normals)
   {
-    int64_t b0[3];
-    int nb[3];
-    for(int a = 0; a < 3; ++a)
-    {
-      b0[a] = brick_floor(base[a]);
-      nb[a] = (int)(brick_floor(end[a] - 1) - b0[a] + 1);
-      G.r[a] = (int)(base[a] - b0[a] * STORE_BRICK);
-      G.tb[a] = nb[a];
-    }
-    table = store_brick_table(v->store->index, b0, nb);
+    VOLUME_REQUIRE(normals_pitch >= sizeof(float4) * (size_t)width && normals_pitch % sizeof(float4) == 0,
+                   "bad normals pitch");
+    VOLUME_REQUIRE(((uintptr_t)dev_normals % 16) == 0, "normals must be 16-byte aligned");
   }
   DeviceGuard guard(v->device);
-  const size_t m = (size_t)dims[0] * (size_t)dims[1] * (size_t)dims[2];
-  int rc = esdf_reserve(v, m, true, table.size(), what);
+  VolumeRaycastParams P = raycast_params(v, width, height, fx, fy, cx, cy, T_curr_world, dev_depth, depth_pitch);
+  VolumeRaycastColour C;
+  memset(&C, 0, sizeof(C));
+  int rc = volume_box_records(v, lo, dims, P.g, dev_intensity ? &C.col : NULL, what);
   if(rc) return rc;
-  if(lookup)
+  // the existing kernels on the box's grid; each writes the plain rays' depth, so both may run
+  if(dev_intensity || !dev_normals)
   {
-    // pageable source: the copy is staged before the call returns
-    RMD_CUDA_TRY(cudaMemcpyAsync(v->esdf_table, table.data(), sizeof(int) * table.size(), cudaMemcpyHostToDevice,
-                                 v->stream));
-    G.table = v->esdf_table;
-    G.pool = v->store->pool;
+    if(dev_intensity)
+    {
+      C.intensity = dev_intensity; C.intensity_stride = intensity_pitch / sizeof(float);
+    }
+    RMD_CUDA_TRY(launch_volume_raycast(P, C, v->stream));
   }
-  G.out = v->esdf_rec;
-  RMD_CUDA_TRY(launch_volume_esdf_gather(G, v->stream));
-  VolumeGrid B = v->g;
-  B.vox = v->esdf_rec;
-  B.nx = dims[0]; B.ny = dims[1]; B.nz = dims[2];
-  const float og[3] = {v->g.ox, v->g.oy, v->g.oz};
-  float o[3];
-  for(int a = 0; a < 3; ++a)   // lo = 0: the window's origin itself
-    o[a] = lo[a] == 0 ? og[a] : shifted_origin(v->o0[a], base[a], v->g.voxel);
-  B.ox = o[0]; B.oy = o[1]; B.oz = o[2];
-  return esdf_passes(v, B, base, o);
+  if(dev_normals)
+  {
+    VolumeRaycastNormals N;
+    N.normals = reinterpret_cast<float4*>(dev_normals);
+    N.normals_stride = normals_pitch / sizeof(float4);
+    RMD_CUDA_TRY(launch_volume_raycast_normals(P, N, v->stream));
+  }
+  return 0;
 }
 
 int rmd_volume_esdf_info(rmd_volume_t *v, int64_t lo_unbounded[3], int dims[3], float origin[3])

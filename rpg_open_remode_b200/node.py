@@ -33,6 +33,71 @@ def esdf_camera_box(dims, voxel_size: float, origin, camera_centre, margin: int)
     return lo, np.maximum(n, c + int(margin) + 1) - lo
 
 
+def _unit_max(u, X, Y):
+    """max of u . q over the unit directions q of the pixel cone {l (x, y, 1): x in [X0, X1], y in [Y0, Y1], l > 0}:
+    a linear function on a spherical polygon peaks at a corner ray, at u's own direction projected onto a side plane
+    when that lies within the side, or at u's direction when that lies within the cone."""
+    (X0, X1), (Y0, Y1) = X, Y
+    cands = [np.array([x, y, 1.0]) for x in (X0, X1) for y in (Y0, Y1)]
+    # the side x = X: the plane spanned by (X, 0, 1) and (0, 1, 0); likewise y = Y
+    for X_ in (X0, X1):
+        nrm = np.array([1.0, 0.0, -X_])
+        p = u - (u @ nrm) / (nrm @ nrm) * nrm
+        if p[2] > 0.0 and Y0 <= p[1] / p[2] <= Y1:
+            cands.append(p)
+    for Y_ in (Y0, Y1):
+        nrm = np.array([0.0, 1.0, -Y_])
+        p = u - (u @ nrm) / (nrm @ nrm) * nrm
+        if p[2] > 0.0 and X0 <= p[0] / p[2] <= X1:
+            cands.append(p)
+    if u[2] > 0.0 and X0 <= u[0] / u[2] <= X1 and Y0 <= u[1] / u[2] <= Y1:
+        cands.append(u)
+    return max(float(u @ c) / float(np.linalg.norm(c)) for c in cands if np.linalg.norm(c) > 0.0)
+
+
+def prior_view_box(dims, voxel_size: float, origin, camera, width: int, height: int, T_world_ref, max_depth: float):
+    """DepthmapNode's prior box with prior_view_box=True: (lo int64 [3], dims int64 [3]) in window indices of the
+    smallest box of whole voxels that contains the camera centre c and every point c + t q for the unit ray q of any
+    pixel position in [0, width - 1] x [0, height - 1] and t in [0, max_depth + voxel_size], plus one voxel on every
+    face for the trilinear corners (DESIGN.md 4.8).  dims: the window's (checked; the box does not depend on them);
+    camera: (fx, fy, cx, cy) or a PinholeCamera; T_world_ref: 3x4 camera -> world.  Float64 throughout, from closed-form
+    extremes per world axis, with esdf_camera_box's conversion to window indices.  The camera centre lies inside the
+    box, so the rays the box prior marches start at the camera and are sampled at t = k * voxel_size whatever the
+    box."""
+    n = np.asarray(dims).reshape(-1)
+    if len(n) != 3 or any(int(x) != x or x <= 0 for x in n):
+        raise ValueError("prior_view_box: dims must be three whole numbers > 0")
+    s = float(voxel_size)
+    if not (np.isfinite(s) and s > 0.0):
+        raise ValueError("prior_view_box: voxel_size must be finite and > 0")
+    o = np.asarray(origin, np.float32).astype(np.float64).reshape(-1)
+    if len(o) != 3 or not np.all(np.isfinite(o)):
+        raise ValueError("prior_view_box: origin must be three finite numbers")
+    fx, fy, cx, cy = ((camera.fx, camera.fy, camera.cx, camera.cy) if hasattr(camera, "fx")
+                      else (float(x) for x in camera))
+    if not all(np.isfinite([fx, fy, cx, cy])) or fx == 0.0 or fy == 0.0:
+        raise ValueError("prior_view_box: the camera needs finite intrinsics and fx, fy != 0")
+    if int(width) != width or int(height) != height or width < 1 or height < 1:
+        raise ValueError("prior_view_box: width and height must be whole numbers >= 1")
+    T = np.asarray(getattr(T_world_ref, "data", T_world_ref), np.float64).reshape(3, 4)
+    if not np.all(np.isfinite(T)):
+        raise ValueError("prior_view_box: T_world_ref must be finite")
+    if not (np.isfinite(max_depth) and max_depth > 0.0):
+        raise ValueError("prior_view_box: max_depth must be finite and > 0")
+    X = sorted(((0.0 - cx) / fx, (width - 1.0 - cx) / fx))
+    Y = sorted(((0.0 - cy) / fy, (height - 1.0 - cy) / fy))
+    R, c = T[:, :3], T[:, 3]
+    reach = float(max_depth) + s
+    lo_w, hi_w = np.empty(3), np.empty(3)
+    for a in range(3):
+        u = R[a]   # (R q)_a = u . q
+        lo_w[a] = c[a] + reach * min(0.0, -_unit_max(-u, X, Y))
+        hi_w[a] = c[a] + reach * max(0.0, _unit_max(u, X, Y))
+    lo = np.floor((lo_w - o) / s).astype(np.int64) - 1
+    hi = np.ceil((hi_w - o) / s).astype(np.int64) + 1
+    return lo, hi - lo + 1
+
+
 class DepthmapNode:
     """rmd::DepthmapNode::denseInputCallback with the ROS plumbing removed.  `publisher` receives
     ("depthmap_and_pointcloud", depthmap) after a keyframe is finished (denoiseAndPublishResults,
@@ -42,7 +107,10 @@ class DepthmapNode:
     def __init__(self, depthmap: Depthmap, ref_compl_perc: float = 10.0, max_dist_from_ref: float = 0.5,
                  publish_conv_every_n: int = 10, publisher: Optional[Callable] = None,
                  volume: Optional[TsdfVolume] = None, prior_from_volume: float = 0.0, follow_volume: bool = False,
-                 scene_mesh: Optional[SceneMesh] = None, esdf: bool = False, esdf_camera_margin: int = 0):
+                 scene_mesh: Optional[SceneMesh] = None, esdf: bool = False, esdf_camera_margin: int = 0,
+                 prior_view_box: bool = False):
+        if prior_view_box and not prior_from_volume:
+            raise ValueError("DepthmapNode: prior_view_box needs prior_from_volume > 0")
         if esdf_camera_margin and not esdf:
             raise ValueError("DepthmapNode: esdf_camera_margin needs esdf=True")
         if int(esdf_camera_margin) != esdf_camera_margin or esdf_camera_margin < 0:
@@ -64,6 +132,9 @@ class DepthmapNode:
         self.volume_ = volume   # when given, every finished keyframe is fused into it (DESIGN.md 4.8)
         # sigma^2 fraction of the new keyframe's prior raycast from volume_ (0 = off)
         self.prior_from_volume_ = float(prior_from_volume)
+        # when set, that raycast marches the box around the new keyframe's view (prior_view_box), brick store
+        # included, instead of the window
+        self.prior_view_box_ = bool(prior_view_box)
         # when set, volume_ is shifted to stay around each keyframe's view before it is fused (DESIGN.md 4.8), and
         # the surface that leaves it is published as ("volume_spill", (points, intensity or None, normals))
         self.follow_volume_ = bool(follow_volume)
@@ -94,7 +165,8 @@ class DepthmapNode:
                 self.state_ = UPDATE                                              # :126-135
                 self.ref_depth_range_ = (float(min_depth), float(max_depth))
                 if self.prior_from_volume_:   # the volume holds every keyframe published so far
-                    self.depthmap_.priorFromVolume(self.volume_, self.prior_from_volume_)
+                    box = self.priorViewBox(max_depth) if self.prior_view_box_ else (None, None)
+                    self.depthmap_.priorFromVolume(self.volume_, self.prior_from_volume_, *box)
         elif self.state_ == UPDATE:
             self.depthmap_.update(img_8uc1, T_curr_world)                         # :142
             perc_conv = self.depthmap_.getConvergedPercentage()                   # :143
@@ -133,6 +205,12 @@ class DepthmapNode:
         T = np.asarray(self.depthmap_.getT_world_ref().data, np.float64).reshape(3, 4)
         return esdf_camera_box(v.dims, v.voxel_size, v.origin, T[:, 3], self.esdf_camera_margin_)
 
+
+    def priorViewBox(self, max_depth: float):
+        """prior_view_box of the keyframe just set: its camera, image and pose, and max_depth."""
+        v, g = self.volume_, self.depthmap_.seeds_
+        T = np.asarray(self.depthmap_.getT_world_ref().data, np.float64).reshape(3, 4)
+        return prior_view_box(v.dims, v.voxel_size, v.origin, g.cam_, g.width_, g.height_, T, max_depth)
 
     def followVolume(self) -> None:
         """Recentre volume_ on the finished keyframe's view centre -- the camera centre plus the middle of
